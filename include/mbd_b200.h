@@ -161,7 +161,8 @@ typedef struct mbd_step_params { uint32_t key[2]; float sigma; float coef[5]; } 
 typedef struct mbd_step_ctl {      /* 128 bytes, zero-initialised by the caller except `i` */
   int32_t i;                       /* current step index (Ndiffuse-1 ... 1) */
   uint32_t epoch;                  /* cross-GPU rendezvous counter (advanced once per step) */
-  uint32_t err;                    /* set to 1 when a cross-GPU rendezvous timed out (outputs are NaN-poisoned) */
+  uint32_t err;                    /* 1: a cross-GPU rendezvous timed out (outputs are NaN-poisoned); 2: a step was launched with
+                                    * i < 1, past the end of the solve (launches 2 and 3 returned without writing anything) */
   uint32_t pad;
   uint32_t ticket[28];             /* "last CTA done" tickets: per column block, [27] over the column blocks... see step_tail.cuh */
 } mbd_step_ctl;
@@ -195,6 +196,10 @@ typedef struct mbd_step_plan {
   uint64_t timeout_cycles;           /* cross-GPU rendezvous timeout in SM cycles; 0 = default (~20 s) */
 } mbd_step_plan;
 int mbd_step_launch(const mbd_step_plan* plan, mbd_stream s);
+/* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
+ * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
+ * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */
+int mbd_step_tail_launch(const mbd_step_plan* plan, mbd_stream s);
 /* the same three launches with CUDA events (mbd_event_create; NULL = skip) recorded before (1), between (1) and (2), between
  * (2) and (3), after (3): lets a caller time each kernel inside the real step on the launching stream (bench.py's roofline
  * and its per-kernel breakdown at every rank count) */

@@ -147,6 +147,13 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
   const int N = a.N;
   const float fN = (float)N;
   const int step = a.ctl->i;
+  // step counter already at 0 (a step launched past the end of the solve): writing rew_hist[step] and, in k_step_update,
+  // Ybars[step - 1] would land outside the tables.  Every CTA reads the same ctl->i (only launch 3 changes it), so the
+  // return is uniform across the cluster and no CTA is left waiting in a cl.sync().
+  if (step < 1) {
+    if (g == 0) a.ctl->err = 2u;
+    return;
+  }
   bool ok = true;
   if (a.P > 1) {
     // rendezvous #1 of the step (flag row 0), then pull every rank's returns over NVLink into rews_all / logpd_all
@@ -309,6 +316,11 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
   const int HNu = a.HNu;
   const int nruns = gridDim.x;
   const int step = a.ctl->i;
+  // past step 1 (see k_step_weights): no CTA writes anything, takes a ticket or moves the counter
+  if (step < 1) {
+    if (blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) a.ctl->err = 2u;
+    return;
+  }
   {
     const int r = blockIdx.x;
     const int n0 = r * kTailRun, n1 = min(n0 + kTailRun, a.n_local);

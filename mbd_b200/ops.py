@@ -211,6 +211,12 @@ def step_launch(plan: "_lib.StepPlan"):
     check(_lib.lib().mbd_step_launch(ctypes.byref(plan), _stream()), "mbd_step_launch")
 
 
+def step_tail_launch(plan: "_lib.StepPlan"):
+    """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
+    buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""
+    check(_lib.lib().mbd_step_tail_launch(ctypes.byref(plan), _stream()), "mbd_step_tail_launch")
+
+
 def ffma_peak(device: Optional[torch.device] = None, iters: int = 4096) -> float:
     """measured fp32 FFMA throughput of the device in TFLOP/s (the fp32 roofline denominator)"""
     _lib.require_gpu()

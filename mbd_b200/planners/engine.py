@@ -224,9 +224,14 @@ class DiffusionEngine:
         return g
 
     def check_exchange(self):
-        """Raises if a cross-GPU rendezvous ever timed out (a peer died or diverged; the outputs are NaN-poisoned).
-        Synchronises: call it outside the step loop."""
-        if int(self.ctl[2].item()) != 0:
+        """Raises if the device reported an error (`mbd_step_ctl.err`): a cross-GPU rendezvous timed out (a peer died or
+        diverged; the outputs are NaN-poisoned), or a step ran with the step counter already at 0 (one `step()` or graph
+        replay too many; the tail kernels then write nothing).  Synchronises: call it outside the step loop."""
+        err = int(self.ctl[2].item())
+        if err == 2:
+            raise ops.MbdError("the step counter ran past step 1 (a step was launched after the last one of the solve); "
+                               "that step wrote nothing")
+        if err != 0:
             raise ops.MbdError("cross-GPU rendezvous timed out (a peer rank stopped participating); outputs are NaN")
 
     @classmethod
