@@ -196,6 +196,15 @@ typedef struct mbd_step_plan {
   uint64_t timeout_cycles;           /* cross-GPU rendezvous timeout in SM cycles; 0 = default (~20 s) */
 } mbd_step_plan;
 int mbd_step_launch(const mbd_step_plan* plan, mbd_stream s);
+/* B independent solves of one env and shape in lockstep: three launches, graph-capturable.  Every per-problem buffer of
+ * `plan` holds B consecutive single-problem blocks (state_init [B][state], params [B][Ndiffuse], ctl [B],
+ * Ybars [B][Ndiffuse][HNu], rew_hist [B][Ndiffuse], Y0s [B][N][HNu], rews / logpd / logp / weights [B][N],
+ * runs [B][nruns][HNu], scalars [B][4]); plan->n_total = n_local = N, n_begin = 0, P = 1.
+ * temps_dev [B] or NULL (= plan->temp for every problem).  car_params / xref are shared by all problems.  Problem b draws
+ * the noise of a stand-alone solve with its own key and reduces in the same order, so it reproduces mbd_step_launch on
+ * its own buffers bit for bit.  MBD_EINVAL (with mbd_last_error) before any CUDA call for B < 1, P != 1, Ndiffuse < 2 or
+ * a plan mbd_step_launch would refuse. */
+int mbd_batch_step_launch(const mbd_step_plan* plan, int B, int Ndiffuse, const float* temps_dev, mbd_stream s);
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

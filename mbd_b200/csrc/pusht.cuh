@@ -19,6 +19,7 @@ struct PushTArgs {
   float* rewss; float* rews; float* final_state; float* traj;
   int fused; uint32_t k0, k1; int n_total, n_begin; float sigma; const float* Ybar;
   const mbd_step_params* sp; const mbd_step_ctl* ctl; const float* Ybars;   // device-resident step parameters (see RolloutArgs)
+  int nd;                                                                     // rows of sp / Ybars per problem (see Problem)
   int prng_part;
 };
 
@@ -278,16 +279,17 @@ __global__ void __launch_bounds__(64) k_pusht(PushTArgs a) {
   const int HNu = a.H * MBD_PT_NU;
   const int nsub = (int)P[MBD_PT_NSUB];
   const uint32_t total = a.prng_part ? 0u : (uint32_t)a.n_total * (uint32_t)HNu;
+  const Problem pb = problem_of(a, blockIdx.y, a.x0, MBD_PT_STATE, HNu);   // problem blockIdx.y of a batch (mbd_b200.cu)
   uint32_t ck0 = a.k0, ck1 = a.k1; float csigma = a.sigma; const float* cYbar = a.Ybar;
   if (a.sp != nullptr) {
-    const int si = a.ctl->i;
-    ck0 = a.sp[si].key[0]; ck1 = a.sp[si].key[1]; csigma = a.sp[si].sigma; cYbar = a.Ybars + (size_t)si * HNu;
+    const int si = pb.ctl->i;
+    ck0 = pb.sp[si].key[0]; ck1 = pb.sp[si].key[1]; csigma = pb.sp[si].sigma; cYbar = pb.Ybars + (size_t)si * HNu;
   }
   float q[MBD_PT_NQ], qd[MBD_PT_NQ];
-  for (int k = 0; k < MBD_PT_NQ; ++k) { q[k] = a.x0[k]; qd[k] = a.x0[MBD_PT_NQ + k]; }
+  for (int k = 0; k < MBD_PT_NQ; ++k) { q[k] = pb.state_init[k]; qd[k] = pb.state_init[MBD_PT_NQ + k]; }
   float sum = 0.0f;
   for (int t = 0; t < a.H; ++t) {
-    float* ur = a.Y0s + ((size_t)i * a.H + t) * 2;
+    float* ur = pb.Y0s + ((size_t)i * a.H + t) * 2;
     float u0, u1;
     if (a.fused) {
       const uint32_t idx = (uint32_t)(a.n_begin + i) * (uint32_t)HNu + (uint32_t)(2 * t);
@@ -307,7 +309,7 @@ __global__ void __launch_bounds__(64) k_pusht(PushTArgs a) {
       for (int k = 0; k < MBD_PT_NQ; ++k) { o[k] = q[k]; o[MBD_PT_NQ + k] = qd[k]; }
     }
   }
-  a.rews[i] = sum / (float)a.H;
+  out_row<true>(a.rews, a.n)[i] = sum / (float)a.H;
   if (a.final_state)
     for (int k = 0; k < MBD_PT_NQ; ++k) { a.final_state[(size_t)i * MBD_PT_STATE + k] = q[k]; a.final_state[(size_t)i * MBD_PT_STATE + MBD_PT_NQ + k] = qd[k]; }
 }

@@ -20,6 +20,10 @@
 //
 // Determinism: every reduction order is a function of (N, n_local / 64) only — never of the rank count — so sharded and
 // unsharded runs agree bit for bit whenever N/P is 64 * 2^k (same guarantee as round 1).
+//
+// Batches (mbd_batch_step_launch, P == 1): problem b of B is blockIdx.y of k_step_weights (B clusters) and blockIdx.z of
+// k_step_update.  Every per-problem buffer holds B consecutive single-problem blocks; each CTA rebases its pointers once at
+// entry and then runs the single-problem code unchanged, so problem b reproduces its stand-alone solve bit for bit.
 #pragma once
 
 #include <cooperative_groups.h>
@@ -63,6 +67,9 @@ struct TailArgs {
   int P, rank;
   unsigned long long off_rews, off_logpd, off_partial, off_flags;   // word offsets in the symmetric buffer
   unsigned long long timeout_cycles;
+  // batches (appended, so that the single-problem fields keep their places in the parameter bank)
+  const float* temps;     // [B] per-problem temperatures, or null (= temp for every problem)
+  int nd;                 // Ndiffuse: the rows of sp / Ybars / rew_hist per problem
 };
 
 __device__ __forceinline__ void tail_st_release_sys(unsigned int* p, unsigned int v) {
@@ -93,6 +100,19 @@ __device__ __forceinline__ bool peer_rendezvous(const TailArgs& a, int row, unsi
 }
 
 enum { TOP_SUM = 0, TOP_MAX = 1 };
+
+// The problem index of a batched launch.  Every kernel that takes part in a batch is instantiated twice from the same source:
+// BATCH = false (every single-problem launch, and B == 1) folds the index to 0, so that code is exactly the single-solve
+// kernel (a runtime index of 0 is not free: rebasing through blockIdx.y cost the packed rollout kernel 7 % on an H100);
+// BATCH = true reads blockIdx.y / blockIdx.z.  batch_y reads the special register afresh at every use: a volatile read is
+// neither hoisted nor kept in a register across the loops between two uses.
+template <bool BATCH>
+__device__ __forceinline__ unsigned batch_y() {
+  if constexpr (!BATCH) return 0u;
+  unsigned v;
+  asm volatile("mov.u32 %0, %%ctaid.y;" : "=r"(v));
+  return v;
+}
 
 // deterministic block reduction (butterfly inside the warp, then warp 0 over the warp results); every thread gets the result
 template <int OP>
@@ -136,6 +156,7 @@ __device__ __forceinline__ float cluster_reduce(float v, float* sh, float* slots
 
 // mbd_planner.py:110-127.  One cluster; thread g of the 8192 cluster threads owns the elements i = g (mod 8192): it re-reads
 // only its own elements in every pass, so the passes need no memory barrier beyond the reductions themselves.
+template <bool BATCH>
 __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsThreads, 1) k_step_weights(TailArgs a) {
   __shared__ float sh[32];
   __shared__ float slots[16];
@@ -146,19 +167,29 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
   constexpr int G = kClusterCtas * kWeightsThreads;
   const int N = a.N;
   const float fN = (float)N;
-  const int step = a.ctl->i;
+  // problem blockIdx.y of a batch (cluster blockIdx.y): its slice of every per-problem buffer (all offsets 0 for one problem)
+  const size_t b = BATCH ? blockIdx.y : 0;
+  mbd_step_ctl* const ctl = a.ctl + b;
+  float* const rews_all = a.rews_all + b * N;
+  float* const logpd_all = a.logpd_all != nullptr ? a.logpd_all + b * N : nullptr;
+  float* const logp = a.logp + b * N;
+  float* const weights = a.weights + b * a.n_local;
+  float* const scalars = a.scalars + 4 * b;
+  float* const rew_hist = a.rew_hist != nullptr ? a.rew_hist + b * a.nd : nullptr;
+  const float temp = a.temps != nullptr ? a.temps[b] : a.temp;
+  const int step = ctl->i;
   // step counter already at 0 (a step launched past the end of the solve): writing rew_hist[step] and, in k_step_update,
   // Ybars[step - 1] would land outside the tables.  Every CTA reads the same ctl->i (only launch 3 changes it), so the
   // return is uniform across the cluster and no CTA is left waiting in a cl.sync().
   if (step < 1) {
-    if (g == 0) a.ctl->err = 2u;
+    if (g == 0) ctl->err = 2u;
     return;
   }
   bool ok = true;
   if (a.P > 1) {
     // rendezvous #1 of the step (flag row 0), then pull every rank's returns over NVLink into rews_all / logpd_all
     if (cl.block_rank() == 0) {
-      bool mine = peer_rendezvous(a, 0, 2u * a.ctl->epoch + 1u);
+      bool mine = peer_rendezvous(a, 0, 2u * ctl->epoch + 1u);
       int all = __syncthreads_and(mine ? 1 : 0);
       if (threadIdx.x == 0) s_ok = all;
     }
@@ -182,14 +213,14 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
       for (int k = 0; k < 8; ++k) {
         const int i = i0 + k * G;
         if (i < N) {
-          a.rews_all[i] = vr[k];
-          if (a.demo) a.logpd_all[i] = vl[k];
+          rews_all[i] = vr[k];
+          if (a.demo) logpd_all[i] = vl[k];
         }
       }
     }
-    if (!ok && g == 0) a.ctl->err = 1u;
+    if (!ok && g == 0) ctl->err = 1u;
   }
-  const float* rews = a.rews_all;
+  const float* rews = rews_all;
   float acc = 0.0f;
   for (int i = g; i < N; i += G) acc += rews[i];
   const float rew_mean = cluster_reduce<TOP_SUM>(acc, sh, slots, &bcast, 0, cl) / fN;
@@ -197,17 +228,16 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
   for (int i = g; i < N; i += G) { float d = rews[i] - rew_mean; acc = fmaf(d, d, acc); }
   float rew_std = sqrtf(cluster_reduce<TOP_SUM>(acc, sh, slots, &bcast, 1, cl) / fN);   // population std (ddof 0)
   rew_std = rew_std < 1e-4f ? 1.0f : rew_std;
-  float* logp = a.logp;
   int pass = 2;
   if (a.demo) {
-    const float* logpd = a.logpd_all;
+    const float* logpd = logpd_all;
     float mxd = -INFINITY;
     for (int i = g; i < N; i += G) mxd = fmaxf(mxd, logpd[i]);
     mxd = cluster_reduce<TOP_MAX>(mxd, sh, slots, &bcast, pass++, cl);
     acc = 0.0f;
     for (int i = g; i < N; i += G) {
-      float l0 = (rews[i] - rew_mean) / rew_std / a.temp;
-      float ld = ((logpd[i] - mxd) + a.rew_xref - rew_mean) / rew_std / a.temp;
+      float l0 = (rews[i] - rew_mean) / rew_std / temp;
+      float ld = ((logpd[i] - mxd) + a.rew_xref - rew_mean) / rew_std / temp;
       float l = ld > l0 ? ld : l0;
       logp[i] = l;
       acc += l;
@@ -216,9 +246,9 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
     acc = 0.0f;
     for (int i = g; i < N; i += G) { float d = logp[i] - lmean; acc = fmaf(d, d, acc); }
     const float lstd = sqrtf(cluster_reduce<TOP_SUM>(acc, sh, slots, &bcast, pass++, cl) / fN);
-    for (int i = g; i < N; i += G) logp[i] = (logp[i] - lmean) / lstd / a.temp;
+    for (int i = g; i < N; i += G) logp[i] = (logp[i] - lmean) / lstd / temp;
   } else {
-    for (int i = g; i < N; i += G) logp[i] = (rews[i] - rew_mean) / rew_std / a.temp;
+    for (int i = g; i < N; i += G) logp[i] = (rews[i] - rew_mean) / rew_std / temp;
   }
   float mx = -INFINITY;
   for (int i = g; i < N; i += G) mx = fmaxf(mx, logp[i]);
@@ -228,11 +258,11 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
   const float S = cluster_reduce<TOP_SUM>(acc, sh, slots, &bcast, pass++, cl);
   for (int i = g; i < N; i += G) {
     const int j = i - a.n_begin;
-    if (j >= 0 && j < a.n_local) a.weights[j] = mbd_expf(logp[i] - mx) / S;
+    if (j >= 0 && j < a.n_local) weights[j] = mbd_expf(logp[i] - mx) / S;
   }
   if (g == 0) {
-    a.scalars[0] = rew_mean; a.scalars[1] = rew_std; a.scalars[2] = mx; a.scalars[3] = S;
-    if (a.rew_hist) a.rew_hist[step] = rew_mean;
+    scalars[0] = rew_mean; scalars[1] = rew_std; scalars[2] = mx; scalars[3] = S;
+    if (rew_hist) rew_hist[step] = rew_mean;
   }
   cl.sync();   // no CTA may exit while its shared memory can still be read by a peer CTA
 }
@@ -308,22 +338,30 @@ __device__ __forceinline__ float diffusion_update(float Ybar, float Ybar_i, cons
   return Yim1 / p.coef[4];
 }
 
-// grid (nruns, ceil(HNu / 256)); block 256.  ctl->ticket[y]: per column block y; ctl->ticket[MBD_STEP_MAX_COLBLOCKS]: over the column blocks.
+// grid (nruns, ceil(HNu / 256), B); block 256.  ctl->ticket[y]: per column block y; ctl->ticket[MBD_STEP_MAX_COLBLOCKS]: over the
+// column blocks.  Problem b = blockIdx.z of a batch uses its own control block, so its tickets and step counter are its own.
+// Its offset is folded into the row / column indices rather than into rebased pointers: the bases stay in the constant bank and
+// the kernel keeps the register count (and so the 8 CTAs per SM) of the single-problem launch.  The host keeps B * N * H * Nu
+// below 2^31, so the int indices cannot overflow.
+template <bool BATCH>
 __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
   __shared__ int s_flag;
   const int tid = threadIdx.x;
   const int j = blockIdx.y * kUpdThreads + tid;
   const int HNu = a.HNu;
   const int nruns = gridDim.x;
-  const int step = a.ctl->i;
+  const int b = BATCH ? blockIdx.z : 0;
+  mbd_step_ctl* const ctl = a.ctl + b;
+  const int step = ctl->i;
   // past step 1 (see k_step_weights): no CTA writes anything, takes a ticket or moves the counter
   if (step < 1) {
-    if (blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) a.ctl->err = 2u;
+    if (blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) ctl->err = 2u;
     return;
   }
   {
     const int r = blockIdx.x;
-    const int n0 = r * kTailRun, n1 = min(n0 + kTailRun, a.n_local);
+    const int nb = b * a.n_local;   // problem b's first sample row
+    const int n0 = nb + r * kTailRun, n1 = nb + min(r * kTailRun + kTailRun, a.n_local);
     if (j < HNu) {
       const float* __restrict__ w = a.weights;
       const float* __restrict__ Y = a.Y0s;
@@ -337,45 +375,46 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
 #pragma unroll
         for (int k = 1; k < 16; ++k) acc = fmaf(w[n0 + k], y[k], acc);
 #pragma unroll
-        for (int b = 16; b < kTailRun; b += 16) {
+        for (int q = 16; q < kTailRun; q += 16) {
 #pragma unroll
-          for (int k = 0; k < 16; ++k) y[k] = Y[(size_t)(n0 + b + k) * HNu + j];
+          for (int k = 0; k < 16; ++k) y[k] = Y[(size_t)(n0 + q + k) * HNu + j];
 #pragma unroll
-          for (int k = 0; k < 16; ++k) acc = fmaf(w[n0 + b + k], y[k], acc);
+          for (int k = 0; k < 16; ++k) acc = fmaf(w[n0 + q + k], y[k], acc);
         }
       } else {
         acc = w[n0] * Y[(size_t)n0 * HNu + j];
         for (int n = n0 + 1; n < n1; ++n) acc = fmaf(w[n], Y[(size_t)n * HNu + j], acc);
       }
-      a.runs[(size_t)r * HNu + j] = acc;
+      a.runs[(size_t)(b * nruns + r) * HNu + j] = acc;
     }
   }
   __threadfence();
   __syncthreads();
-  if (tid == 0) s_flag = (atomicAdd(&a.ctl->ticket[blockIdx.y], 1u) == (unsigned)(nruns - 1));
+  if (tid == 0) s_flag = (atomicAdd(&ctl->ticket[blockIdx.y], 1u) == (unsigned)(nruns - 1));
   __syncthreads();
   if (!s_flag) return;
   // ---- last CTA of this column block: every run row of these columns is complete -------------------------------------
   __threadfence();
-  const mbd_step_params p = a.sp[step];
-  float* out = a.Ybars + (size_t)(step - 1) * HNu;
-  const float* Ybar_i = a.Ybars + (size_t)step * HNu;
+  const mbd_step_params p = a.sp[b * a.nd + step];
+  float* out = a.Ybars + (size_t)(b * a.nd + step - 1) * HNu;
+  const float* Ybar_i = out + HNu;
   if (j < HNu) {
-    const float v = tail_tree_rows<false>(nullptr, a.runs, nruns, (size_t)HNu, j);
+    // problem b's run rows start b * nruns rows into the table: the offset goes into the column index
+    const float v = tail_tree_rows<false>(nullptr, a.runs, nruns, (size_t)HNu, j + b * nruns * HNu);
     if (a.P == 1) out[j] = diffusion_update(v, Ybar_i[j], p);
     else a.partial[j] = v;
   }
-  if (tid == 0) a.ctl->ticket[blockIdx.y] = 0u;
+  if (tid == 0) ctl->ticket[blockIdx.y] = 0u;
   __threadfence();
   __syncthreads();
-  if (tid == 0) s_flag = (atomicAdd(&a.ctl->ticket[MBD_STEP_MAX_COLBLOCKS], 1u) == gridDim.y - 1);
+  if (tid == 0) s_flag = (atomicAdd(&ctl->ticket[MBD_STEP_MAX_COLBLOCKS], 1u) == gridDim.y - 1);
   __syncthreads();
   if (!s_flag) return;
   // ---- the very last CTA of the launch ----------------------------------------------------------------------------------
   __threadfence();
   if (a.P > 1) {
     // rendezvous #2 (flag row 1): every rank's partial is complete; fold them in rank order and apply the update
-    bool mine = peer_rendezvous(a, 1, 2u * a.ctl->epoch + 2u);
+    bool mine = peer_rendezvous(a, 1, 2u * ctl->epoch + 2u);
     const bool ok = __syncthreads_and(mine ? 1 : 0) != 0;
     const float* bases[8];
 #pragma unroll
@@ -384,13 +423,13 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
       const float v = tail_tree_rows<true>(bases, nullptr, a.P, 0, c);
       out[c] = ok ? diffusion_update(v, Ybar_i[c], p) : __int_as_float(0x7fc00000);
     }
-    if (!ok && tid == 0) a.ctl->err = 1u;
+    if (!ok && tid == 0) ctl->err = 1u;
   }
   __syncthreads();
   if (tid == 0) {
-    a.ctl->ticket[MBD_STEP_MAX_COLBLOCKS] = 0u;
-    a.ctl->epoch = a.ctl->epoch + 1u;
-    a.ctl->i = step - 1;
+    ctl->ticket[MBD_STEP_MAX_COLBLOCKS] = 0u;
+    ctl->epoch = ctl->epoch + 1u;
+    ctl->i = step - 1;
   }
 }
 

@@ -211,6 +211,12 @@ def step_launch(plan: "_lib.StepPlan"):
     check(_lib.lib().mbd_step_launch(ctypes.byref(plan), _stream()), "mbd_step_launch")
 
 
+def batch_step_launch(plan: "_lib.StepPlan", B: int, Ndiffuse: int, temps: Optional[torch.Tensor] = None):
+    """one diffusion step of B independent problems in lockstep (mbd_batch_step_launch): every per-problem buffer of `plan`
+    holds B consecutive single-problem blocks; temps [B] on the device, or None for plan.temp everywhere"""
+    check(_lib.lib().mbd_batch_step_launch(ctypes.byref(plan), int(B), int(Ndiffuse), _p(temps), _stream()), "mbd_batch_step_launch")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

@@ -69,6 +69,45 @@ def key_chain(rng_exp, Ndiffuse: int) -> np.ndarray:
     return keys
 
 
+def pack_step_params(keys: np.ndarray, sigmas: np.ndarray, alphas: np.ndarray, alphas_bar: np.ndarray) -> np.ndarray:
+    """The device table of a whole solve (`mbd_step_params` rows, as int32 words): row i = {Y0s_rng of step i, sigmas[i],
+    update_coef(i)}.  Row 0 carries the key and sigma only (step 0 is never run)."""
+    Nd = len(sigmas)
+    if keys.shape != (Nd, 2):
+        raise ops.MbdError(f"key chain of shape {keys.shape} does not match a schedule of {Nd} steps")
+    tab = np.zeros((Nd, _lib.STEP_PARAMS_WORDS), np.uint32)
+    tab[:, 0:2] = keys
+    tab[:, 2] = np.asarray(sigmas, np.float32).view(np.uint32)
+    for i in range(1, Nd):
+        tab[i, 3:8] = np.asarray(update_coef(alphas, alphas_bar, i), np.float32).view(np.uint32)
+    return tab.view(np.int32)
+
+
+def env_tensors(env, state_init, enable_demo: bool, d: torch.device):
+    """(model, params_car, state_init, xref) of one env on device d: what launch (1) of a step reads.  model is the
+    device-resident blob of a Brax-positional env (None for car2d / pushT, whose table is params_car); xref is the
+    demonstration when enable_demo is set."""
+    if env.kind == "xpbd":
+        raw = state_init.pipeline_state.raw if hasattr(state_init, "pipeline_state") else state_init
+        xref = torch.as_tensor(env.xref, device=d).contiguous() if enable_demo else None
+        return env.device_model(d), None, torch.as_tensor(np.ascontiguousarray(raw, dtype=np.float32), device=d), xref
+    if env.kind == "car2d":
+        params_car, xref = env.device_params()
+        x0 = state_init.pipeline_state if hasattr(state_init, "pipeline_state") else state_init
+        return None, params_car, torch.as_tensor(np.ascontiguousarray(x0, dtype=np.float32), device=d), (xref if enable_demo else None)
+    if env.kind == "pusht":
+        if enable_demo:
+            raise ValueError("pushT has no demonstration (mbd_planner.py:118 applies to humanoidtrack / car2d)")
+        raw = state_init.pipeline_state.raw if hasattr(state_init, "pipeline_state") else state_init
+        return None, env.device_params(), torch.as_tensor(np.ascontiguousarray(raw, dtype=np.float32), device=d), None
+    raise ValueError(env.kind)
+
+
+def xref_len(env, xref) -> int:
+    """href of the step plan: the demonstration's length in steps (0 without one)"""
+    return 0 if xref is None else int(xref.shape[1] if env.kind == "xpbd" else xref.shape[0])
+
+
 class DiffusionEngine:
     def __init__(self, env, Nsample: int, Hsample: int, temp_sample: float, enable_demo: bool, state_init,
                  device: Optional[torch.device] = None, group=None, Ndiffuse: int = 2, emulate=None):
@@ -132,28 +171,7 @@ class DiffusionEngine:
         self.launches_per_step = 3
         self.launches_last_step = 3
         self.graph = None
-        if env.kind == "xpbd":
-            self.model = env.device_model(d)
-            raw = state_init.pipeline_state.raw if hasattr(state_init, "pipeline_state") else state_init
-            self.state_init = torch.as_tensor(np.ascontiguousarray(raw, dtype=np.float32), device=d)
-            self.xref = torch.as_tensor(env.xref, device=d).contiguous() if self.enable_demo else None
-            self.params_car = None
-        elif env.kind == "car2d":
-            self.model = None
-            self.params_car, xref = env.device_params()
-            x0 = state_init.pipeline_state if hasattr(state_init, "pipeline_state") else state_init
-            self.state_init = torch.as_tensor(np.ascontiguousarray(x0, dtype=np.float32), device=d)
-            self.xref = xref if self.enable_demo else None
-        elif env.kind == "pusht":
-            if self.enable_demo:
-                raise ValueError("pushT has no demonstration (mbd_planner.py:118 applies to humanoidtrack / car2d)")
-            self.model = None
-            self.params_car = env.device_params()
-            raw = state_init.pipeline_state.raw if hasattr(state_init, "pipeline_state") else state_init
-            self.state_init = torch.as_tensor(np.ascontiguousarray(raw, dtype=np.float32), device=d)
-            self.xref = None
-        else:
-            raise ValueError(env.kind)
+        self.model, self.params_car, self.state_init, self.xref = env_tensors(env, state_init, self.enable_demo, d)
         self.rew_xref = float(getattr(env, "rew_xref", 0.0))
         self._plan_c = self._make_plan()
 
@@ -169,7 +187,7 @@ class DiffusionEngine:
         p.temp, p.rew_xref = self.temp, self.rew_xref
         p.xref_dev = vp(self.xref)
         p.env_kind = _lib.ENV_PUSHT if self.env.kind == "pusht" else _lib.ENV_CAR2D
-        p.href = 0 if self.xref is None else int(self.xref.shape[1] if self.env.kind == "xpbd" else self.xref.shape[0])
+        p.href = xref_len(self.env, self.xref)
         p.Y0s_dev, p.rews_dev, p.logpd_dev = vp(self.Y0s), vp(self.rews_local), vp(self.logpd_local)
         p.rews_all_dev, p.logpd_all_dev, p.logp_dev = vp(self.rews_all), vp(self.logpd_all), vp(self.logp_scratch)
         p.weights_dev, p.runs_dev, p.partial_dev, p.scalars_dev = vp(self.weights), vp(self.run_scratch), vp(self.partial), vp(self.scalars)
@@ -186,12 +204,7 @@ class DiffusionEngine:
         Nd = self.Nd
         if len(sigmas) != Nd or keys.shape != (Nd, 2):
             raise ops.MbdError(f"schedule of {len(sigmas)} steps does not match the engine (Ndiffuse={Nd})")
-        tab = np.zeros((Nd, _lib.STEP_PARAMS_WORDS), np.uint32)
-        tab[:, 0:2] = keys
-        tab[:, 2] = np.asarray(sigmas, np.float32).view(np.uint32)
-        for i in range(1, Nd):
-            tab[i, 3:8] = np.asarray(update_coef(alphas, alphas_bar, i), np.float32).view(np.uint32)
-        self.params.copy_(torch.from_numpy(tab.view(np.int32)))
+        self.params.copy_(torch.from_numpy(pack_step_params(keys, sigmas, alphas, alphas_bar)))
 
     def set_step(self, i: int):
         """device step counter <- i (the next `step()` runs diffusion step i: reads Ybars[i], writes Ybars[i-1])"""
@@ -299,3 +312,119 @@ class DiffusionEngine:
             out.copy_(res)
             res = out
         return res, self.scalars[0]
+
+
+class BatchedDiffusionEngine:
+    """B independent solves of one env and shape (N, H, Ndiffuse, demo) stepped in lockstep: ONE three-launch step
+    (`mbd_batch_step_launch`) advances all of them.  Problem b has its own initial state, key chain, schedule (beta0 / betaT
+    may differ) and temperature; every per-problem device buffer is [B, ...] with problem b's single-solve block at index b.
+    The noise of problem b is drawn from its own key with problem-local counters and every reduction order depends on N only,
+    so problem b reproduces the `DiffusionEngine` solve of the same inputs bit for bit.  One GPU (P = 1)."""
+
+    def __init__(self, env, Nsample: int, Hsample: int, temps, enable_demo: bool, state_inits, Ndiffuse: int,
+                 device: Optional[torch.device] = None):
+        self.env = env
+        self.B = len(state_inits)
+        if self.B < 1 or len(temps) != self.B:
+            raise ValueError(f"{self.B} initial states and {len(temps)} temperatures: need one of each per problem, B >= 1")
+        self.N, self.H = int(Nsample), int(Hsample)
+        self.enable_demo = bool(enable_demo)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.Nu = env.action_size
+        self.HNu = self.H * self.Nu
+        self.Nd = int(Ndiffuse)
+        if self.Nd < 2:
+            raise ValueError("Ndiffuse must be at least 2")
+        B, N, d = self.B, self.N, self.device
+        f = dict(device=d, dtype=torch.float32)
+        per = [env_tensors(env, s, self.enable_demo, d) for s in state_inits]
+        self.model, self.params_car, _, self.xref = per[0]              # shared by every problem
+        self.state_init = torch.stack([p[2] for p in per]).contiguous()  # [B, state]
+        self.temps = torch.tensor(np.asarray(temps, np.float32), device=d)
+        self.Y0s = torch.empty((B, N, self.HNu), **f)
+        self.rews = torch.empty((B, N), **f)
+        self.logpd = torch.empty((B, N), **f) if self.enable_demo else None
+        self.logp_scratch = torch.empty((B, N), **f)
+        self.weights = torch.empty((B, N), **f)
+        self.scalars = torch.zeros((B, 4), **f)
+        self.run_scratch = torch.empty((B, (N + ops.RUN - 1) // ops.RUN, self.HNu), **f)
+        self.partial = torch.empty(self.HNu, **f)                       # read by sharded steps only; the plan requires it
+        self.Ybars = torch.zeros((B, self.Nd, self.HNu), **f)
+        self.rew_hist = torch.zeros((B, self.Nd), **f)
+        self.params = torch.zeros((B, self.Nd, _lib.STEP_PARAMS_WORDS), device=d, dtype=torch.int32)
+        self.ctl = torch.zeros((B, _lib.STEP_CTL_WORDS), device=d, dtype=torch.int32)
+        self.rew_xref = float(getattr(env, "rew_xref", 0.0))
+        self.graph = None
+        self._plan_c = self._make_plan()
+
+    def _make_plan(self) -> "_lib.StepPlan":
+        p = _lib.StepPlan()
+        vp = lambda t: None if t is None else t.data_ptr()   # noqa: E731
+        p.model = self.model._h if self.model is not None else None
+        p.car_params_dev, p.state_init_dev = vp(self.params_car), vp(self.state_init)
+        p.params_dev, p.ctl_dev, p.Ybars_dev, p.rew_hist_dev = vp(self.params), vp(self.ctl), vp(self.Ybars), vp(self.rew_hist)
+        p.n_total, p.n_begin, p.n_local, p.H, p.nu = self.N, 0, self.N, self.H, self.Nu
+        p.temp, p.rew_xref = 0.0, self.rew_xref      # the per-problem temperatures come from self.temps
+        p.xref_dev = vp(self.xref)
+        p.env_kind = _lib.ENV_PUSHT if self.env.kind == "pusht" else _lib.ENV_CAR2D
+        p.href = xref_len(self.env, self.xref)
+        p.Y0s_dev, p.rews_dev, p.logpd_dev = vp(self.Y0s), vp(self.rews), vp(self.logpd)
+        p.rews_all_dev, p.logpd_all_dev, p.logp_dev = vp(self.rews), vp(self.logpd), vp(self.logp_scratch)
+        p.weights_dev, p.runs_dev, p.partial_dev, p.scalars_dev = vp(self.weights), vp(self.run_scratch), vp(self.partial), vp(self.scalars)
+        p.P, p.rank = 1, 0
+        return p
+
+    # ---- solve-level API (that of DiffusionEngine, one entry per problem) -----------------------------------------------
+    def load_schedule(self, keys, sigmas, alphas, alphas_bar):
+        """uploads every problem's solve: keys[b] [Ndiffuse, 2] (key_chain), sigmas[b] / alphas[b] / alphas_bar[b] (make_schedule)"""
+        if not (len(keys) == len(sigmas) == len(alphas) == len(alphas_bar) == self.B):
+            raise ops.MbdError(f"need {self.B} key chains and schedules, one per problem")
+        for b in range(self.B):
+            if len(sigmas[b]) != self.Nd:
+                raise ops.MbdError(f"problem {b}: schedule of {len(sigmas[b])} steps does not match the engine (Ndiffuse={self.Nd})")
+        tab = np.stack([pack_step_params(np.asarray(keys[b]), sigmas[b], alphas[b], alphas_bar[b]) for b in range(self.B)])
+        self.params.copy_(torch.from_numpy(tab))
+
+    def set_step(self, i: int):
+        """every problem's device step counter <- i"""
+        self.ctl[:, 0].fill_(int(i))
+
+    def step(self):
+        """one diffusion step of every problem (three launches, or one replay of the captured graph)"""
+        if self.graph is not None:
+            self.graph.replay()
+        else:
+            ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)
+
+    def capture(self):
+        """records one batched step in a CUDA graph; later `step()` calls replay it"""
+        i0 = self.ctl[:, 0].clone()
+        s = torch.cuda.Stream(device=self.device)
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)   # warm-up outside capture
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        self.ctl[:, 0].copy_(i0)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)
+        self.graph = g
+        return g
+
+    def check_exchange(self):
+        """Raises if any problem's control block reports an error, naming the problems: err 2 = a step ran with the step
+        counter already at 0 (one `step()` or replay too many; that step wrote nothing).  Synchronises."""
+        err = self.ctl[:, 2].cpu().numpy()
+        bad = [int(b) for b in np.nonzero(err)[0]]
+        if not bad:
+            return
+        if all(int(err[b]) == 2 for b in bad):
+            raise ops.MbdError(f"problems {bad}: the step counter ran past step 1 (a step was launched after the last one of "
+                               "the solve); that step wrote nothing")
+        raise ops.MbdError(f"problems {bad}: device error codes {[int(err[b]) for b in bad]}")
+
+    def problem(self, b: int):
+        """the single-problem view of problem b that `final_reward` and the rollout helpers take (model, tables, state_init)"""
+        from types import SimpleNamespace
+        return SimpleNamespace(model=self.model, params_car=self.params_car, state_init=self.state_init[b], H=self.H, Nu=self.Nu)

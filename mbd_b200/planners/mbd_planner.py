@@ -16,7 +16,7 @@ import torch.distributed as dist
 
 import mbd_b200
 from mbd_b200 import ops, prng
-from mbd_b200.planners.engine import DiffusionEngine, key_chain, make_schedule
+from mbd_b200.planners.engine import BatchedDiffusionEngine, DiffusionEngine, key_chain, make_schedule
 
 try:  # tqdm is cosmetic
     from tqdm import tqdm
@@ -131,6 +131,68 @@ def run_diffusion(args: Args, log_every: int = 10, return_trajectory: bool = Fal
     rew_final = final_reward(env, engine, Yi[-1])
     if return_trajectory:
         return rew_final, Yi
+    return rew_final
+
+
+# fields every problem of one run_diffusion_batch call must share (one env and shape); seed, temp_sample, beta0 and betaT may differ
+BATCH_SHARED_FIELDS = ("env_name", "Nsample", "Hsample", "Ndiffuse", "enable_demo")
+
+
+def check_batch_args(args_list) -> None:
+    """The argument checks of run_diffusion_batch, before anything touches the device: raises ValueError naming the field.
+    Expects the recommended parameters already applied."""
+    if len(args_list) < 1:
+        raise ValueError("run_diffusion_batch needs at least one Args")
+    for a in args_list:
+        if not a.not_render:
+            raise ValueError("run_diffusion_batch requires not_render=True (it writes no artefacts)")
+    for f in BATCH_SHARED_FIELDS:
+        vals = [getattr(a, f) for a in args_list]
+        if any(v != vals[0] for v in vals):
+            raise ValueError(f"run_diffusion_batch: every problem must have the same {f} (got {vals})")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1 or (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+        raise ValueError("run_diffusion_batch runs on one GPU; it cannot run under WORLD_SIZE > 1")
+
+
+def run_diffusion_batch(args_list, log_every: int = 10, return_trajectory: bool = False):
+    """run_diffusion for B problems of one env and shape at once: ONE three-launch step advances all of them
+    (BatchedDiffusionEngine).  Each problem's reset, key chain and schedule come from its own Args exactly as in
+    run_diffusion, so problem b returns the rew_final of run_diffusion(args_list[b]) bit for bit.  Returns np.ndarray[B] of
+    rew_final (and with return_trajectory the list of every problem's Yi).  Requires not_render=True; one GPU only."""
+    for a in args_list:
+        apply_recommended_params(a)
+    check_batch_args(args_list)
+    a0 = args_list[0]
+    env = mbd_b200.envs.get_env(a0.env_name)
+    Nu = env.action_size
+    state_inits, keys, scheds = [], [], []
+    for a in args_list:
+        rng = prng.PRNGKey(seed=a.seed)
+        rng, rng_reset = prng.split(rng)  # NOTE: rng_reset should never be changed.
+        state_inits.append(env.reset(rng_reset))
+        betas, alphas, alphas_bar, sigmas = make_schedule(a.beta0, a.betaT, a.Ndiffuse)
+        print(f"init sigma = {sigmas[-1]:.2e}")
+        rng_exp, rng = prng.split(rng)
+        keys.append(key_chain(rng_exp, a.Ndiffuse))
+        scheds.append((sigmas, alphas, alphas_bar))
+    engine = BatchedDiffusionEngine(env, a0.Nsample, a0.Hsample, [a.temp_sample for a in args_list], a0.enable_demo, state_inits,
+                                    a0.Ndiffuse)
+    engine.load_schedule(keys, [s[0] for s in scheds], [s[1] for s in scheds], [s[2] for s in scheds])
+    engine.set_step(a0.Ndiffuse - 1)
+    if os.environ.get("MBD_GRAPH", "1") != "0":
+        engine.capture()
+    steps = range(a0.Ndiffuse - 1, 0, -1)
+    pbar = tqdm(steps, desc=f"Diffusing x{engine.B}") if tqdm is not None else None
+    for n_done, i in enumerate(pbar if pbar is not None else steps):
+        engine.step()
+        if pbar is not None and (n_done % log_every == log_every - 1 or i == 1):
+            pbar.set_postfix({"rew": f"{engine.rew_hist[:, i].mean().item():.2e}"})   # mean over the problems
+            engine.check_exchange()
+    engine.check_exchange()
+    Yis = [engine.Ybars[b, : a0.Ndiffuse - 1].flip(0).reshape(a0.Ndiffuse - 1, a0.Hsample, Nu) for b in range(engine.B)]
+    rew_final = np.array([final_reward(env, engine.problem(b), Yis[b][-1]) for b in range(engine.B)])
+    if return_trajectory:
+        return rew_final, Yis
     return rew_final
 
 
