@@ -147,7 +147,9 @@ template <class T> PK_FN void axis_angle_1dof(Q<T> j, T& psi, T& r10, T& r20) {
   r20 = mul(two, fma(x, z, neg(mul(w, y))));
   psi = atan2_(neg(r12), r22);
 }
-template <class T> PK_FN void axis_angle_ang(Q<T> j, T parity, Angles<T>& o) {
+// third = false leaves ang[2] / ax[2] unset: phase A of a 2-dof joint never reads them, and their atan2_ is ~10 % of
+// that phase's issue (phase C needs all three: the locked third axis enters dqj).  Warp-uniform, so a uniform branch.
+template <class T> PK_FN void axis_angle_ang(Q<T> j, T parity, Angles<T>& o, bool third = true) {
   const T zero = bc<T>(0.0f), one = bc<T>(1.0f), two = bc<T>(2.0f);
   T w = j.w, x = j.x, y = j.y, z = j.z;
   T r00 = sub_nf(one, mul(two, fma(z, z, mul(y, y))));
@@ -160,13 +162,16 @@ template <class T> PK_FN void axis_angle_ang(Q<T> j, T parity, Angles<T>& o) {
   T psi = atan2_(neg(r12), r22);
   T cth = sqrt_(fma(r01, r01, mul(r00, r00)));
   T theta = atan2_(r02, cth);
-  T phi = atan2_(neg(r01), r00);
   T ln;
   V<T> lon = vnormalize(mkV(zero, r22, neg(r12)), &ln);
-  o.ang[0] = psi; o.ang[1] = theta; o.ang[2] = mul(parity, phi);
+  o.ang[0] = psi; o.ang[1] = theta;
   o.ax[0] = mkV(one, zero, zero);
   o.ax[1] = lon;
-  o.ax[2] = mkV(mul(parity, r02), mul(parity, r12), mul(parity, r22));
+  if (third) {
+    T phi = atan2_(neg(r01), r00);
+    o.ang[2] = mul(parity, phi);
+    o.ax[2] = mkV(mul(parity, r02), mul(parity, r12), mul(parity, r22));
+  }
 }
 
 // ---- contacts against the z = 0 plane (xpbd_device.cuh::contact_position_plane / contact_velocity_plane) ----------------
@@ -257,7 +262,7 @@ PK_FN void phase_A(const Model<T>& M, const Cfg& c, const Smem<T>& S, State<T>& 
       tq = vfma(mkV(one, zero, zero), t, tq);
     } else {
       Angles<T> ja;
-      axis_angle_ang(j, M.l(MBD_F_PARITY, c.l), ja);
+      axis_angle_ang(j, M.l(MBD_F_PARITY, c.l), ja, c.ndof > 2);
 #if PK_DEVICE
 #pragma unroll
 #endif
