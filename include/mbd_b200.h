@@ -131,7 +131,9 @@ int mbd_peer_gather(const uint64_t* peer_base_ptrs, int P, int rank, size_t src_
                     size_t flag_off_words, uint32_t epoch, float* dst_dev, uint32_t* err_dev, mbd_stream s);
 
 /* Test hook: element-wise MBD_DIV (op 0), MBD_RCP (1), MBD_SQRT (2), mbd_atan2f (3) — the branch-free
- * exact device sequences of include/mbd_fp32.h — so tests can compare them with IEEE results bit for bit. */
+ * exact device sequences of include/mbd_fp32.h — so tests can compare them with IEEE results bit for bit; and the
+ * packed rollout kernel's atan2_ (csrc/pk_scalar.cuh): its scalar instantiation (4) and its two-lane f2 instantiation with
+ * element i in the low (5) or the high (6) half, element n-1-i in the other. */
 int mbd_test_arith(int op, const float* a_dev, const float* b_dev, float* out_dev, int n, mbd_stream s);
 
 /* Ybar = tree-sum of the P rank partials; then score / Yim1 / Ybar_im1 literally as

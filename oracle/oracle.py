@@ -112,6 +112,16 @@ def simd_rollout(blob, state_init, Y0s, want_final=False, nthreads=0):
     return dict(rews=rews, final=final, logpd=None, rewss=None, track=None)
 
 
+def build_variant(defs: dict, out: str):
+    """Builds the oracle with other values of its ORC_* switches (oracle/Makefile `variant`) into `out` and loads it.
+    Swap it in for the default library with `oracle._LIB = build_variant(...)`."""
+    flags = " ".join(f"-D{k}={v}" for k, v in defs.items())
+    subprocess.run(["make", "-C", _HERE, "variant", f"DEFS={flags}", f"OUT={out}"], check=True, capture_output=True)
+    L = ctypes.CDLL(out)
+    L.orc_num_threads.restype = ctypes.c_int
+    return L
+
+
 def lib():
     global _LIB
     if _LIB is None:

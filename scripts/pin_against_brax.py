@@ -24,10 +24,8 @@ Exit code 0 with the line "PARITY UNPINNED: brax is not importable" when Brax is
 from __future__ import annotations
 
 import argparse
-import ctypes
 import itertools
 import os
-import subprocess
 import sys
 import tempfile
 
@@ -54,12 +52,7 @@ PT_SWITCHES = {"ORC_PT_REG_INVWEIGHT": [0, 1], "ORC_PT_CONTACT_MIDPOINT": [1, 0]
 FIELDS = [("x_i.pos", slice(0, 3)), ("x_i.rot", slice(3, 7)), ("xd_i.ang", slice(7, 10)), ("xd_i.vel", slice(10, 13))]
 
 
-def build_variant(defs: dict, out: str):
-    flags = " ".join(f"-D{k}={v}" for k, v in defs.items())
-    subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "variant", f"DEFS={flags}", f"OUT={out}"], check=True, capture_output=True)
-    L = ctypes.CDLL(out)
-    L.orc_num_threads.restype = ctypes.c_int
-    return L
+from oracle.oracle import build_variant  # noqa: E402  (shared with tests/test_xpbd_ref_cpu.py)
 
 
 def step_states(lib, blob, states, action):

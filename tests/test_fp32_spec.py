@@ -10,16 +10,38 @@ def _ulp_err(got, ref):
 
 
 def test_atan2(orc):
+    """mbd_atan2f within ATAN2_ULP ulps of float64 atan2 — the bound the float64 reference of the positional step
+    (tests/xpbd_ref.py) charges every Euler angle — over the operand ranges the Euler extraction produces"""
+    from tests.xpbd_ref import ATAN2_ULP
     rng = np.random.default_rng(0)
+    f64 = lambda a: a.astype(np.float64)   # noqa: E731
     y = rng.normal(size=100000).astype(np.float32)
     x = rng.normal(size=100000).astype(np.float32)
-    assert _ulp_err(orc.fmap("atan2", y, x), np.arctan2(y.astype(np.float64), x.astype(np.float64))) <= 4.0
-    # axes, signs and zeros
-    yy = np.float32([0, 0, 1, -1, 0.0, 1e-30, -1e-30, 3, -3])
-    xx = np.float32([1, -1, 0, 0, 0.0, 1, -1, 3, -3])
+    assert _ulp_err(orc.fmap("atan2", y, x), np.arctan2(f64(y), f64(x))) <= ATAN2_ULP
+    # |y/x| from 1e-30 to 1e30 in all four quadrants, |x| from 1e-3 to 1e3
+    n = 400000
+    x = (10.0 ** rng.uniform(-3, 3, n)) * rng.choice([-1.0, 1.0], n)
+    y = np.abs(x) * 10.0 ** rng.uniform(-30, 30, n) * rng.choice([-1.0, 1.0], n)
+    x, y = x.astype(np.float32), y.astype(np.float32)
+    assert _ulp_err(orc.fmap("atan2", y, x), np.arctan2(f64(y), f64(x))) <= ATAN2_ULP
+    # y = +-x over the whole normal range
+    x = ((10.0 ** rng.uniform(-30, 30, n)) * rng.choice([-1.0, 1.0], n)).astype(np.float32)
+    for y in (x, -x):
+        assert _ulp_err(orc.fmap("atan2", y, x), np.arctan2(f64(y), f64(x))) <= ATAN2_ULP
+    # axes: exact
+    yy = np.float32([0, 0, 1, -1, 3e-30, -3e-30])
+    xx = np.float32([1, -1, 0, 0, 0, 0])
     got = orc.fmap("atan2", yy, xx)
-    ref = np.arctan2(yy.astype(np.float64), xx.astype(np.float64))
-    assert np.allclose(got, ref, atol=3e-7)
+    assert got.tolist() == [0.0, np.float32(np.pi), np.float32(np.pi / 2), -np.float32(np.pi / 2), np.float32(np.pi / 2), -np.float32(np.pi / 2)]
+    # signed zeros: the sign tests are `x < 0` and `y < 0`, so a negative zero counts as positive.  atan2(-0, x > 0) is +0
+    # (IEEE: -0), atan2(-0, x < 0) is +pi (IEEE: -pi) and atan2(+-0, +-0) is +0 (IEEE: +-0 or +-pi).  The float64 reference
+    # treats an exact zero y with x < 0 as the branch cut (both +-pi).
+    yy = np.float32([0.0, -0.0, 0.0, -0.0, 0.0, -0.0, 0.0, -0.0])
+    xx = np.float32([1.0, 1.0, -1.0, -1.0, 0.0, 0.0, -0.0, -0.0])
+    got = orc.fmap("atan2", yy, xx)
+    pi = np.float32(np.pi)
+    assert got.tolist() == [0.0, 0.0, pi, pi, 0.0, 0.0, 0.0, 0.0]
+    assert not np.signbit(got).any()
 
 
 def test_sincos(orc):

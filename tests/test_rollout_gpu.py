@@ -106,6 +106,9 @@ def test_exact_arith(orc):
     y, xx = mag(-6, 3), mag(-6, 3)
     y[:1000] = 0.0; xx[500:1500] = 0.0
     assert_bit_exact(run(3, y, xx), orc.fmap("atan2", y, xx), "atan2 (device division inside)")
+    # the packed kernel's atan2_ (div_nn_ inside): scalar, and either half of its two-lane instantiation
+    for op, what in ((4, "scalar"), (5, "f2 low half"), (6, "f2 high half")):
+        assert_bit_exact(run(op, y, xx), orc.fmap("atan2", y, xx), f"packed atan2_, {what}")
 
 
 def test_sampling_bit_exact(orc):
