@@ -207,6 +207,31 @@ int mbd_step_launch(const mbd_step_plan* plan, mbd_stream s);
  * its own buffers bit for bit.  MBD_EINVAL (with mbd_last_error) before any CUDA call for B < 1, P != 1, Ndiffuse < 2 or
  * a plan mbd_step_launch would refuse. */
 int mbd_batch_step_launch(const mbd_step_plan* plan, int B, int Ndiffuse, const float* temps_dev, mbd_stream s);
+/* ---- the path-integral baselines (upstream mbd/planners/path_integral.py:33-52) as the same three launches ----------------
+ * B independent refinements of one env and shape in lockstep, laid out exactly as mbd_batch_step_launch (Ndiffuse = Nrefine
+ * rows: Ybars row i = mu_0t of step i, the result goes to row i - 1, rews.mean() to rew_hist[i]).  Launch (1) is unchanged and
+ * reads sigma_t from params[i].sigma; launch (2) computes the softmax weights of path_integral.py:116-124 (and, for CEM, selects
+ * the top 10); launch (3) applies the method's update:
+ *   MBD_PI_MPPI   Ybars[i-1] = sum_n w_n Y_n
+ *   MBD_PI_CMAES  Ybars[i-1] as MPPI; sigma' = max(mean_j sqrt(sum_n w_n (Y_nj - Ybars[i]_j)^2) * sigma_i, 1e-3) (fp32) is written
+ *                 to params[i-1].sigma (read by the next step's launch (1)) and to sigma_hist[i-1]
+ *   MBD_PI_CEM    idx = argsort(w)[::-1][:10] (stable, so equal weights come highest index first); Ybars[i-1] = mean of those rows
+ * A batch of one runs the single-problem (non-batched) kernel instantiations. */
+enum { MBD_PI_MPPI = 1, MBD_PI_CMAES = 2, MBD_PI_CEM = 3 };
+#define MBD_PI_IDX_STRIDE 16 /* ints per problem in cem_idx_dev: slots 0..9 = picked rows in rank order (-1 past the count), 10 = count */
+typedef struct mbd_pi_bufs {        /* 24 bytes */
+  float* sigma_hist_dev;            /* [B][Nrefine]; CMA-ES writes row i - 1 of each step (may be NULL for MPPI / CEM) */
+  float* cma_scratch_dev;           /* CMA-ES: [B][ceil(N/64) + 1][H*Nu] (NULL otherwise) */
+  int32_t* cem_idx_dev;             /* CEM: [B][MBD_PI_IDX_STRIDE] (NULL otherwise) */
+} mbd_pi_bufs;
+/* tail_only != 0: launches (2) and (3) only, on whatever the caller put into Y0s / rews / Ybars[i] / params[i] (tests).
+ * MBD_EINVAL (with mbd_last_error) before any CUDA call for an unknown method, P != 1, Nrefine < 2, B outside 1..65535, a demo
+ * (xref), a missing buffer of the method, or a plan mbd_batch_step_launch would refuse. */
+int mbd_pi_batch_step_launch(const mbd_step_plan* plan, int B, int Nrefine, int method, const float* temps_dev,
+                             const mbd_pi_bufs* bufs, int tail_only, mbd_stream s);
+/* sizeof / offsetof of mbd_pi_bufs (cross-checked against the ctypes mirror) */
+int mbd_pi_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

@@ -45,6 +45,15 @@ class StepPlan(ctypes.Structure):
     ]
 
 
+class PiBufs(ctypes.Structure):
+    """mbd_pi_bufs (include/mbd_b200.h): the buffers the path-integral update rules add to a step plan"""
+    _fields_ = [("sigma_hist_dev", c_vp), ("cma_scratch_dev", c_vp), ("cem_idx_dev", c_vp)]
+
+
+PI_METHODS = {"mppi": 1, "cma-es": 2, "cem": 3}   # MBD_PI_MPPI / MBD_PI_CMAES / MBD_PI_CEM
+PI_IDX_STRIDE = 16       # MBD_PI_IDX_STRIDE: ints per problem in cem_idx (10 picks, then the count)
+PI_TOPK = 10
+
 STEP_PARAMS_WORDS = 8    # sizeof(mbd_step_params) / 4
 STEP_CTL_WORDS = 32      # sizeof(mbd_step_ctl) / 4
 ENV_CAR2D, ENV_PUSHT = 0, 1   # mbd_step_plan.env_kind (model == NULL)
@@ -93,6 +102,9 @@ def lib():
     L.mbd_step_launch.argtypes = [ctypes.POINTER(StepPlan), c_vp]
     L.mbd_step_tail_launch.argtypes = [ctypes.POINTER(StepPlan), c_vp]
     L.mbd_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, c_vp, c_vp]
+    L.mbd_pi_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
+                                           ctypes.POINTER(PiBufs), ctypes.c_int, c_vp]
+    L.mbd_pi_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes = [ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -107,7 +119,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_model_set_group_map", "mbd_set_group_stagger", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

@@ -72,6 +72,24 @@ struct TailArgs {
   int nd;                 // Ndiffuse: the rows of sp / Ybars / rew_hist per problem
 };
 
+// Update rule of the tail (template parameter RULE of k_step_weights / k_step_update).  RULE_MBD is the diffusion update of
+// mbd_planner.py:130-133 and takes TailArgs; the path-integral rules of path_integral.py:33-52 (values = MBD_PI_*) take PiArgs,
+// which appends their buffers, so the MBD instantiations keep their parameter bank.
+enum { RULE_MBD = 0, RULE_MPPI = MBD_PI_MPPI, RULE_CMAES = MBD_PI_CMAES, RULE_CEM = MBD_PI_CEM };
+constexpr int kCemTop = 10;             // path_integral.py:50 `[:10]`
+
+struct PiArgs {
+  TailArgs t;
+  mbd_step_params* sp;    // == t.sp, writable: CMA-ES stores sigma' in row i - 1 for the next step's launch (1)
+  float* sigma_hist;      // [B][nd]: CMA-ES writes sigma' to row i - 1
+  float* sq_runs;         // CMA-ES: [B][nruns + 1][HNu]: the runs of sum_n w_n (Y_n - mu)^2, then one row of their column roots
+  int* cem_idx;           // CEM: [B][MBD_PI_IDX_STRIDE]: the picked rows in rank order, slot kCemTop = their count
+};
+template <int RULE> struct RuleArgs { using type = PiArgs; };
+template <> struct RuleArgs<RULE_MBD> { using type = TailArgs; };
+__device__ __forceinline__ const TailArgs& tail_of(const TailArgs& a) { return a; }
+__device__ __forceinline__ const TailArgs& tail_of(const PiArgs& a) { return a.t; }
+
 __device__ __forceinline__ void tail_st_release_sys(unsigned int* p, unsigned int v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
@@ -154,10 +172,81 @@ __device__ __forceinline__ float cluster_reduce(float v, float* sh, float* slots
   return r;
 }
 
+// CEM selection key of weight w at index i: the weight's bits above i + 1.  Weights are >= 0, so the key order is the order of
+// (w, i); the largest key is the heaviest sample and, among equal weights, the one with the highest index — the order of
+// jnp.argsort (stable, ascending) reversed.  0 is no sample.
+__device__ __forceinline__ unsigned long long cem_key(float w, int i) {
+  return ((unsigned long long)__float_as_uint(w) << 32) | (unsigned)(i + 1);
+}
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, v, o);
+    v = t > v ? t : v;
+  }
+  return v;
+}
+
+// path_integral.py:50, idx = argsort(weights)[::-1][:10], inside k_step_weights once the weights are written.  Keys are unique,
+// so "the k-th largest key" is well defined and every stage below finds the same set: (1) each warp picks its 10 largest keys
+// in 10 rounds (every lane offers its largest key below the previous pick, the warp takes the max); (2) warp 0 picks the
+// CTA's 10 from the 32 x 10 warp picks; (3) after a cluster barrier, warp 0 of CTA 0 reads the 8 x 10 CTA picks over DSMEM and
+// picks the final 10 in rank order.  out[0..9] = indices (-1 past the count), out[kCemTop] = count = min(N, 10).
+template <int G>
+__device__ __forceinline__ void cem_select(const float* w, int N, int g, cg::cluster_group& cl, int* out) {
+  __shared__ unsigned long long s_warp[32 * kCemTop];
+  __shared__ unsigned long long s_cta[kCemTop];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long below = ~0ull;
+  for (int k = 0; k < kCemTop; ++k) {
+    unsigned long long best = 0;
+    for (int i = g; i < N; i += G) {
+      const unsigned long long key = cem_key(w[i], i);
+      if (key < below && key > best) best = key;
+    }
+    below = warp_max_u64(best);
+    if (lane == 0) s_warp[warp * kCemTop + k] = below;
+  }
+  __syncthreads();
+  if (warp == 0) {
+    below = ~0ull;
+    for (int k = 0; k < kCemTop; ++k) {
+      unsigned long long best = 0;
+      for (int q = 0; q < kCemTop; ++q) {
+        const unsigned long long key = s_warp[lane * kCemTop + q];
+        if (key < below && key > best) best = key;
+      }
+      below = warp_max_u64(best);
+      if (lane == 0) s_cta[k] = below;
+    }
+  }
+  cl.sync();
+  if (cl.block_rank() == 0 && warp == 0) {
+    unsigned long long c[kCemTop];
+    const unsigned long long* peer = cl.map_shared_rank(s_cta, lane < kClusterCtas ? lane : 0);
+#pragma unroll
+    for (int q = 0; q < kCemTop; ++q) c[q] = lane < kClusterCtas ? peer[q] : 0ull;
+    below = ~0ull;
+    int count = 0;
+    for (int k = 0; k < kCemTop; ++k) {
+      unsigned long long best = 0;
+#pragma unroll
+      for (int q = 0; q < kCemTop; ++q)
+        if (c[q] < below && c[q] > best) best = c[q];
+      below = warp_max_u64(best);
+      if (lane == 0) out[k] = below != 0 ? (int)(unsigned)(below & 0xffffffffull) - 1 : -1;
+      count += below != 0;
+    }
+    if (lane == 0) out[kCemTop] = count;
+  }
+}
+
 // mbd_planner.py:110-127.  One cluster; thread g of the 8192 cluster threads owns the elements i = g (mod 8192): it re-reads
 // only its own elements in every pass, so the passes need no memory barrier beyond the reductions themselves.
-template <bool BATCH>
-__global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsThreads, 1) k_step_weights(TailArgs a) {
+// The path-integral rules reuse it unchanged (path_integral.py:116-124); RULE_CEM then selects the top 10 (cem_select).
+template <bool BATCH, int RULE = RULE_MBD>
+__global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsThreads, 1)
+    k_step_weights(const typename RuleArgs<RULE>::type args) {
+  const TailArgs& a = tail_of(args);
   __shared__ float sh[32];
   __shared__ float slots[16];
   __shared__ float bcast;
@@ -264,6 +353,7 @@ __global__ void __cluster_dims__(kClusterCtas, 1, 1) __launch_bounds__(kWeightsT
     scalars[0] = rew_mean; scalars[1] = rew_std; scalars[2] = mx; scalars[3] = S;
     if (rew_hist) rew_hist[step] = rew_mean;
   }
+  if constexpr (RULE == RULE_CEM) cem_select<G>(weights, N, g, cl, args.cem_idx + b * MBD_PI_IDX_STRIDE);
   cl.sync();   // no CTA may exit while its shared memory can still be read by a peer CTA
 }
 
@@ -343,8 +433,33 @@ __device__ __forceinline__ float diffusion_update(float Ybar, float Ybar_i, cons
 // Its offset is folded into the row / column indices rather than into rebased pointers: the bases stay in the constant bank and
 // the kernel keeps the register count (and so the 8 CTAs per SM) of the single-problem launch.  The host keeps B * N * H * Nu
 // below 2^31, so the int indices cannot overflow.
-template <bool BATCH>
-__global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
+// CMA-ES term of a run: (y - mu)^2 as k_wsum_runs<true> forms it (path_integral.py:43)
+__device__ __forceinline__ float sqerr_term(float y, float m) {
+  const float d = y - m;
+  return d * d;
+}
+
+// CMA-ES, very last CTA of the launch: sigma' = max(mean_j sqrt(sum_n w_n (Y_nj - mu_j)^2) * sigma_i, 1e-3) (path_integral.py:43-45)
+// in fp32.  Fixed order: thread t adds the roots of columns t, t + 256, t + 512, ... in that order; the 256 thread sums are folded
+// by an xor butterfly inside each warp (offsets 1, 2, 4, 8, 16), then the 8 warp sums by one over offsets 1, 2, 4.
+__device__ __forceinline__ float cma_sigma(const float* roots, int HNu, float sigma_i) {
+  __shared__ float s_red[kUpdThreads / 32];
+  float acc = 0.0f;
+  for (int c = threadIdx.x; c < HNu; c += kUpdThreads) acc += __ldcg(roots + c);   // written by other CTAs of this launch
+  for (int o = 1; o < 32; o <<= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  float r = 0.0f;
+  if (threadIdx.x < 32) {
+    r = threadIdx.x < kUpdThreads / 32 ? s_red[threadIdx.x] : 0.0f;
+    for (int o = 1; o < kUpdThreads / 32; o <<= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+  }
+  return fmaxf((r / (float)HNu) * sigma_i, 1e-3f);
+}
+
+template <bool BATCH, int RULE = RULE_MBD>
+__global__ void __launch_bounds__(kUpdThreads) k_step_update(const typename RuleArgs<RULE>::type args) {
+  const TailArgs& a = tail_of(args);
   __shared__ int s_flag;
   const int tid = threadIdx.x;
   const int j = blockIdx.y * kUpdThreads + tid;
@@ -358,7 +473,7 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
     if (blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) ctl->err = 2u;
     return;
   }
-  {
+  if constexpr (RULE != RULE_CEM) {   // CEM has no weighted sum: one CTA per column block (gridDim.x == 1)
     const int r = blockIdx.x;
     const int nb = b * a.n_local;   // problem b's first sample row
     const int n0 = nb + r * kTailRun, n1 = nb + min(r * kTailRun + kTailRun, a.n_local);
@@ -366,26 +481,41 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
       const float* __restrict__ w = a.weights;
       const float* __restrict__ Y = a.Y0s;
       float acc;
+      // CMA-ES reads Y0s once for both sums; mu_0t is the OLD mean, Ybars row i of problem b (path_integral.py:43)
+      float acc2 = 0.0f, m = 0.0f;
+      if constexpr (RULE == RULE_CMAES) m = a.Ybars[(size_t)(b * a.nd + step) * HNu + j];
       if (n1 - n0 == kTailRun) {
         // full run: 16 loads in flight per thread (the accumulation order stays sequential)
         float y[16];
 #pragma unroll
         for (int k = 0; k < 16; ++k) y[k] = Y[(size_t)(n0 + k) * HNu + j];
         acc = w[n0] * y[0];
+        if constexpr (RULE == RULE_CMAES) acc2 = w[n0] * sqerr_term(y[0], m);
 #pragma unroll
-        for (int k = 1; k < 16; ++k) acc = fmaf(w[n0 + k], y[k], acc);
+        for (int k = 1; k < 16; ++k) {
+          acc = fmaf(w[n0 + k], y[k], acc);
+          if constexpr (RULE == RULE_CMAES) acc2 = fmaf(w[n0 + k], sqerr_term(y[k], m), acc2);
+        }
 #pragma unroll
         for (int q = 16; q < kTailRun; q += 16) {
 #pragma unroll
           for (int k = 0; k < 16; ++k) y[k] = Y[(size_t)(n0 + q + k) * HNu + j];
 #pragma unroll
-          for (int k = 0; k < 16; ++k) acc = fmaf(w[n0 + q + k], y[k], acc);
+          for (int k = 0; k < 16; ++k) {
+            acc = fmaf(w[n0 + q + k], y[k], acc);
+            if constexpr (RULE == RULE_CMAES) acc2 = fmaf(w[n0 + q + k], sqerr_term(y[k], m), acc2);
+          }
         }
       } else {
         acc = w[n0] * Y[(size_t)n0 * HNu + j];
-        for (int n = n0 + 1; n < n1; ++n) acc = fmaf(w[n], Y[(size_t)n * HNu + j], acc);
+        if constexpr (RULE == RULE_CMAES) acc2 = w[n0] * sqerr_term(Y[(size_t)n0 * HNu + j], m);
+        for (int n = n0 + 1; n < n1; ++n) {
+          acc = fmaf(w[n], Y[(size_t)n * HNu + j], acc);
+          if constexpr (RULE == RULE_CMAES) acc2 = fmaf(w[n], sqerr_term(Y[(size_t)n * HNu + j], m), acc2);
+        }
       }
       a.runs[(size_t)(b * nruns + r) * HNu + j] = acc;
+      if constexpr (RULE == RULE_CMAES) args.sq_runs[(size_t)(b * (nruns + 1) + r) * HNu + j] = acc2;
     }
   }
   __threadfence();
@@ -398,11 +528,32 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
   const mbd_step_params p = a.sp[b * a.nd + step];
   float* out = a.Ybars + (size_t)(b * a.nd + step - 1) * HNu;
   const float* Ybar_i = out + HNu;
-  if (j < HNu) {
-    // problem b's run rows start b * nruns rows into the table: the offset goes into the column index
-    const float v = tail_tree_rows<false>(nullptr, a.runs, nruns, (size_t)HNu, j + b * nruns * HNu);
-    if (a.P == 1) out[j] = diffusion_update(v, Ybar_i[j], p);
-    else a.partial[j] = v;
+  if constexpr (RULE == RULE_MBD) {
+    if (j < HNu) {
+      // problem b's run rows start b * nruns rows into the table: the offset goes into the column index
+      const float v = tail_tree_rows<false>(nullptr, a.runs, nruns, (size_t)HNu, j + b * nruns * HNu);
+      if (a.P == 1) out[j] = diffusion_update(v, Ybar_i[j], p);
+      else a.partial[j] = v;
+    }
+  } else if constexpr (RULE == RULE_CEM) {
+    // path_integral.py:51, mu = mean(Y0s[idx]): the picked rows added in rank order, then divided by their count
+    const int* idx = args.cem_idx + b * MBD_PI_IDX_STRIDE;
+    const int cnt = idx[kCemTop];
+    if (j < HNu) {
+      const float* Y = a.Y0s + (size_t)b * a.n_local * HNu + j;
+      float s = Y[(size_t)idx[0] * HNu];
+      for (int k = 1; k < cnt; ++k) s += Y[(size_t)idx[k] * HNu];
+      out[j] = s / (float)cnt;
+    }
+  } else {
+    if (j < HNu) {
+      // MPPI / CMA-ES mean (path_integral.py:35, :42): the tree value itself, no schedule lines
+      out[j] = tail_tree_rows<false>(nullptr, a.runs, nruns, (size_t)HNu, j + b * nruns * HNu);
+      if constexpr (RULE == RULE_CMAES) {
+        float* sq = args.sq_runs + (size_t)b * (nruns + 1) * HNu;
+        sq[(size_t)nruns * HNu + j] = sqrtf(tail_tree_rows<false>(nullptr, sq, nruns, (size_t)HNu, j));
+      }
+    }
   }
   if (tid == 0) ctl->ticket[blockIdx.y] = 0u;
   __threadfence();
@@ -424,6 +575,13 @@ __global__ void __launch_bounds__(kUpdThreads) k_step_update(TailArgs a) {
       out[c] = ok ? diffusion_update(v, Ybar_i[c], p) : __int_as_float(0x7fc00000);
     }
     if (!ok && tid == 0) ctl->err = 1u;
+  }
+  if constexpr (RULE == RULE_CMAES) {
+    const float sg = cma_sigma(args.sq_runs + ((size_t)b * (nruns + 1) + nruns) * HNu, HNu, p.sigma);
+    if (tid == 0) {
+      args.sp[b * a.nd + step - 1].sigma = sg;
+      args.sigma_hist[b * a.nd + step - 1] = sg;
+    }
   }
   __syncthreads();
   if (tid == 0) {

@@ -217,6 +217,14 @@ def batch_step_launch(plan: "_lib.StepPlan", B: int, Ndiffuse: int, temps: Optio
     check(_lib.lib().mbd_batch_step_launch(ctypes.byref(plan), int(B), int(Ndiffuse), _p(temps), _stream()), "mbd_batch_step_launch")
 
 
+def pi_batch_step_launch(plan: "_lib.StepPlan", B: int, Nrefine: int, method: int, temps: Optional[torch.Tensor],
+                         bufs: "_lib.PiBufs", tail_only: bool = False):
+    """one path-integral refinement step (MPPI / CMA-ES / CEM, `method` = _lib.PI_METHODS[name]) of B problems in lockstep
+    (mbd_pi_batch_step_launch), laid out as batch_step_launch; tail_only: launches 2 and 3 on the inputs already in the buffers"""
+    check(_lib.lib().mbd_pi_batch_step_launch(ctypes.byref(plan), int(B), int(Nrefine), int(method), _p(temps), ctypes.byref(bufs),
+                                              int(bool(tail_only)), _stream()), "mbd_pi_batch_step_launch")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

@@ -69,16 +69,17 @@ def key_chain(rng_exp, Ndiffuse: int) -> np.ndarray:
     return keys
 
 
-def pack_step_params(keys: np.ndarray, sigmas: np.ndarray, alphas: np.ndarray, alphas_bar: np.ndarray) -> np.ndarray:
+def pack_step_params(keys: np.ndarray, sigmas: np.ndarray, alphas: Optional[np.ndarray], alphas_bar: Optional[np.ndarray]) -> np.ndarray:
     """The device table of a whole solve (`mbd_step_params` rows, as int32 words): row i = {Y0s_rng of step i, sigmas[i],
-    update_coef(i)}.  Row 0 carries the key and sigma only (step 0 is never run)."""
+    update_coef(i)}.  Row 0 carries the key and sigma only (step 0 is never run).  alphas None (the path-integral baselines,
+    which have no schedule): every coefficient is 0."""
     Nd = len(sigmas)
     if keys.shape != (Nd, 2):
         raise ops.MbdError(f"key chain of shape {keys.shape} does not match a schedule of {Nd} steps")
     tab = np.zeros((Nd, _lib.STEP_PARAMS_WORDS), np.uint32)
     tab[:, 0:2] = keys
     tab[:, 2] = np.asarray(sigmas, np.float32).view(np.uint32)
-    for i in range(1, Nd):
+    for i in range(1, Nd if alphas is not None else 0):
         tab[i, 3:8] = np.asarray(update_coef(alphas, alphas_bar, i), np.float32).view(np.uint32)
     return tab.view(np.int32)
 
@@ -394,7 +395,11 @@ class BatchedDiffusionEngine:
         if self.graph is not None:
             self.graph.replay()
         else:
-            ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)
+            self._launch()
+
+    def _launch(self):
+        """the three launches of one step of every problem"""
+        ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)
 
     def capture(self):
         """records one batched step in a CUDA graph; later `step()` calls replay it"""
@@ -402,13 +407,13 @@ class BatchedDiffusionEngine:
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
-            ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)   # warm-up outside capture
+            self._launch()   # warm-up outside capture
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self.ctl[:, 0].copy_(i0)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)
+            self._launch()
         self.graph = g
         return g
 

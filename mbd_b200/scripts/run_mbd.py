@@ -5,7 +5,12 @@
 algo=mbd runs the eight problems of a sweep as ONE batch (run_diffusion_batch): one three-launch step advances all of them,
 and each problem's result equals its stand-alone run_diffusion bit for bit.  The `time:` line then reports the batch's wall
 clock divided by the batch size (the problems are not timed one by one).  algo=path_integral calls run_path_integral once per
-seed or temperature, as the reference does.
+seed or temperature, as the reference does; with --pi_batch it runs the eight as ONE batch (run_path_integral_batch) and reports
+the batch's wall clock divided by B, like algo=mbd.
+
+The path_integral temperature sweep keeps the reference's quirk: it builds Args(seed=0, env_name, temp_sample=t) without
+disable_recommended_params and without update_method, so for an env of the recommended-parameter table every problem runs at the
+recommended temperature, and every temperature runs MPPI.  The batch builds the same eight Args.
 """
 from __future__ import annotations
 
@@ -26,6 +31,7 @@ class Args:
     update_method: str = "mppi"  # softmax, cma-es, cem
     mode: str = "seed"  # temp
     env_name: str = "ant"
+    pi_batch: bool = False  # algo=path_integral: run the sweep as one batch (run_path_integral_batch)
 
 
 def seed_args(args: Args):
@@ -37,13 +43,26 @@ def temp_args(args: Args):
             for t in TEMPS]
 
 
-def _run_mbd_batch(args_list):
+def pi_seed_args(args: Args):
+    return [path_integral.Args(seed=s, env_name=args.env_name, update_method=args.update_method) for s in SEEDS]
+
+
+def pi_temp_args(args: Args):
+    """the reference's quirk: no disable_recommended_params, no update_method (see the module docstring)"""
+    return [path_integral.Args(seed=0, env_name=args.env_name, temp_sample=float(t)) for t in TEMPS]
+
+
+def _run_batch(run, args_list):
     """(rews [B], seconds per problem): the batch's wall clock, synchronised, divided by B"""
     import torch
     t0 = time()
-    rews = mbd_planner.run_diffusion_batch(args_list)
+    rews = run(args_list)
     torch.cuda.synchronize()
     return np.asarray(rews), (time() - t0) / len(args_list)
+
+
+def _run_mbd_batch(args_list):
+    return _run_batch(mbd_planner.run_diffusion_batch, args_list)
 
 
 def run_multiple_seed(args: Args):
@@ -54,10 +73,15 @@ def run_multiple_seed(args: Args):
         return rews
     if args.algo != "path_integral":
         raise NotImplementedError(args.algo)
+    if args.pi_batch:
+        rews, per = _run_batch(path_integral.run_path_integral_batch, pi_seed_args(args))
+        print(f"rew: {rews.mean():.2f} \\pm {rews.std():.2f}")
+        print(f"time: {per:.2f} \\pm {0.0:.2f} (wall clock of one batch of {len(rews)} / {len(rews)})")
+        return rews
     rews, times = [], []
-    for seed in SEEDS:
+    for pa in pi_seed_args(args):
         t0 = time()
-        rews.append(path_integral.run_path_integral(path_integral.Args(seed=seed, env_name=args.env_name, update_method=args.update_method)))
+        rews.append(path_integral.run_path_integral(pa))
         times.append(time() - t0)
     rews, times = np.array(rews), np.array(times)
     print(f"rew: {rews.mean():.2f} \\pm {rews.std():.2f}")
@@ -69,9 +93,10 @@ def run_multiple_temp(args: Args):
     temps = np.array(TEMPS)
     if args.algo == "mbd":
         rews, _ = _run_mbd_batch(temp_args(args))
+    elif args.algo == "path_integral" and args.pi_batch:
+        rews, _ = _run_batch(path_integral.run_path_integral_batch, pi_temp_args(args))
     elif args.algo == "path_integral":
-        rews = np.array([path_integral.run_path_integral(path_integral.Args(seed=0, env_name=args.env_name, temp_sample=float(t)))
-                         for t in temps])
+        rews = np.array([path_integral.run_path_integral(pa) for pa in pi_temp_args(args)])
     else:
         raise NotImplementedError(args.algo)
     best_temp = temps[np.argmax(rews)]
