@@ -41,8 +41,8 @@ struct PtMinv { float imp, A00, A01, A02, A11, A12, A22; };
 
 // The padded NRP x NRP constraint system and its projected Gauss-Seidel sweeps.  Jc / posc hold the nr ACTIVE rows compacted to
 // the front.  For NRP = 4 and 8 every array below — and Jc itself when the caller built it in registers — is indexed by
-// compile-time constants after unrolling, i.e. lives in registers.  The sweeps stop when none of the multipliers moved by more than
-// MBD_PT_TOL of the largest one (with TOL = 0: at an exact fixed point, where all later sweeps would be no-ops).
+// compile-time constants after unrolling, i.e. lives in registers.  The sweeps stop when a sweep moved the constraint force J^T x by
+// no more than MBD_PT_TOL of its largest component (with TOL = 0: when the sweep left the force exactly unchanged).
 template <int NRP>
 __device__ __forceinline__ void pt_solve(const float* P, const float (*Jc)[5], const float* posc, const float* rsc, int nr, const PtMinv& M,
                                          const float* Mif, const float* qd, int iters, float* xout) {

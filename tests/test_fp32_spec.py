@@ -45,9 +45,20 @@ def test_atan2(orc):
 
 
 def test_sincos(orc):
-    a = np.random.default_rng(1).uniform(-40, 40, size=100000).astype(np.float32)
-    assert np.max(np.abs(orc.fmap("sin", a) - np.sin(a.astype(np.float64)))) < 2.5e-7
-    assert np.max(np.abs(orc.fmap("cos", a) - np.cos(a.astype(np.float64)))) < 2.5e-7
+    """mbd_sincosf within COS_ABS_ERR (absolute) of float64 over |x| <= 1200: the bound tests/xpbd_ref.py and
+    tests/pusht_ref.py charge every sine and cosine, the latter for slider angles up to 1e3 rad"""
+    from tests.xpbd_ref import COS_ABS_ERR
+    rng = np.random.default_rng(1)
+    for hi in (40.0, 1200.0):
+        a = rng.uniform(-hi, hi, size=200000).astype(np.float32)
+        assert np.max(np.abs(orc.fmap("sin", a) - np.sin(a.astype(np.float64)))) < COS_ABS_ERR
+        assert np.max(np.abs(orc.fmap("cos", a) - np.cos(a.astype(np.float64)))) < COS_ABS_ERR
+    # the fp32 neighbours of multiples of pi / 2 (largest reduced argument error) up to 1200
+    k = np.arange(-764, 765)
+    a = np.concatenate([np.nextafter(np.float32(k * np.pi / 2), d) for d in (np.float32(-np.inf), np.float32(np.inf))])
+    a = np.concatenate([a, np.float32(k * np.pi / 2)])
+    assert np.max(np.abs(orc.fmap("sin", a) - np.sin(a.astype(np.float64)))) < COS_ABS_ERR
+    assert np.max(np.abs(orc.fmap("cos", a) - np.cos(a.astype(np.float64)))) < COS_ABS_ERR
 
 
 def test_log_exp(orc):

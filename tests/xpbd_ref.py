@@ -44,7 +44,7 @@ from mbd_b200.model import blob as B
 U = 2.0 ** -24
 ETA = 2.0 ** -149
 ATAN2_ULP = 4.0          # max ulp error of mbd_atan2f; tests/test_fp32_spec.py::test_atan2 proves it
-COS_ABS_ERR = 2.5e-7     # max absolute error of mbd_cosf on |x| <= 40; tests/test_fp32_spec.py::test_sincos
+COS_ABS_ERR = 2.5e-7     # max absolute error of mbd_sincosf on |x| <= 1200; tests/test_fp32_spec.py::test_sincos
 EPS = float(np.float32(1e-6))   # XPBD regulariser (ORC_EPS default)
 ROT_GRAD = 4.5   # |d(R(q) v)/dq| <= (4|radial| + 2|tangential|) |v| <= sqrt(20) |v| near |q| = 1
 ROT_ROUND = 32
