@@ -231,6 +231,25 @@ int mbd_pi_batch_step_launch(const mbd_step_plan* plan, int B, int Nrefine, int 
                              const mbd_pi_bufs* bufs, int tail_only, mbd_stream s);
 /* sizeof / offsetof of mbd_pi_bufs (cross-checked against the ctypes mirror) */
 int mbd_pi_abi_sizes(int32_t* out, int n);
+/* ---- model-based diffusion as a black-box optimiser (upstream mbd/blackbox/mbd_opt.py:64-80) as the same three launches -------
+ * B independent solves of one objective and shape in lockstep, laid out as mbd_batch_step_launch with H = 1 and nu = dim
+ * (model, car_params, state_init and xref are not read and model / xref must be NULL).  Launch (1) (csrc/blackbox.cuh) draws
+ * Y0s = clip(normal(params[i].key, (N, dim)) * params[i].sigma + mu, -1, 1), where mu is Ybars row i or, on the first step
+ * (i == Ndiffuse - 1), the per-sample normal(init_keys[b], (N, dim)) of mbd_opt.py:84; it writes rews = J = -f(Y0s) and folds
+ * max_n J_n into best_hist[b][i].  Launches (2) and (3) are those of MBD_PI_MPPI: Ybars[i-1] = sum_n w_n Y_n.
+ * MBD_EINVAL (with mbd_last_error) before any CUDA call for an unknown fn, P != 1, Ndiffuse < 2, B outside 1..65535, H != 1, a
+ * model or xref in the plan, missing bufs, x_min >= x_max, or a plan mbd_batch_step_launch would refuse (dim > 27 * 256,
+ * N * dim >= 2^32). */
+enum { MBD_BBO_ACKLEY = 1, MBD_BBO_RASTRIGIN = 2, MBD_BBO_LEVY = 3 };
+typedef struct mbd_bbo_bufs {        /* 24 bytes */
+  const uint32_t* init_keys_dev;     /* [B][2]: PRNGKey(seed) of each problem (the first step's per-sample mean) */
+  float* best_hist_dev;              /* [B][Ndiffuse]: row i = max_n J_n of step i; initialised by the caller (-inf) */
+  float x_min, x_max;                /* domain map X = x_min + (x_max - x_min) * (Y + 1) / 2 */
+} mbd_bbo_bufs;
+int mbd_bbo_batch_step_launch(const mbd_step_plan* plan, int B, int Ndiffuse, int fn, const float* temps_dev,
+                              const mbd_bbo_bufs* bufs, mbd_stream s);
+/* sizeof / offsetof of mbd_bbo_bufs and the MBD_BBO_* values (cross-checked against the ctypes mirror) */
+int mbd_bbo_abi_sizes(int32_t* out, int n);
 
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as

@@ -225,6 +225,14 @@ def pi_batch_step_launch(plan: "_lib.StepPlan", B: int, Nrefine: int, method: in
                                               int(bool(tail_only)), _stream()), "mbd_pi_batch_step_launch")
 
 
+def bbo_batch_step_launch(plan: "_lib.StepPlan", B: int, Ndiffuse: int, fn: int, temps: Optional[torch.Tensor],
+                          bufs: "_lib.BboBufs"):
+    """one black-box optimisation step (`fn` = _lib.BBO_FNS[name]) of B problems in lockstep (mbd_bbo_batch_step_launch), laid
+    out as batch_step_launch with H = 1 and nu = dim"""
+    check(_lib.lib().mbd_bbo_batch_step_launch(ctypes.byref(plan), int(B), int(Ndiffuse), int(fn), _p(temps), ctypes.byref(bufs),
+                                               _stream()), "mbd_bbo_batch_step_launch")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

@@ -336,11 +336,16 @@ class BatchedDiffusionEngine:
         self.Nd = int(Ndiffuse)
         if self.Nd < 2:
             raise ValueError("Ndiffuse must be at least 2")
-        B, N, d = self.B, self.N, self.device
-        f = dict(device=d, dtype=torch.float32)
-        per = [env_tensors(env, s, self.enable_demo, d) for s in state_inits]
+        per = [env_tensors(env, s, self.enable_demo, self.device) for s in state_inits]
         self.model, self.params_car, _, self.xref = per[0]              # shared by every problem
         self.state_init = torch.stack([p[2] for p in per]).contiguous()  # [B, state]
+        self.rew_xref = float(getattr(env, "rew_xref", 0.0))
+        self._alloc(temps)
+
+    def _alloc(self, temps):
+        """the per-problem device buffers and the C plan, from B, N, HNu, Nd, enable_demo and the env tensors set before"""
+        B, N, d = self.B, self.N, self.device
+        f = dict(device=d, dtype=torch.float32)
         self.temps = torch.tensor(np.asarray(temps, np.float32), device=d)
         self.Y0s = torch.empty((B, N, self.HNu), **f)
         self.rews = torch.empty((B, N), **f)
@@ -354,7 +359,6 @@ class BatchedDiffusionEngine:
         self.rew_hist = torch.zeros((B, self.Nd), **f)
         self.params = torch.zeros((B, self.Nd, _lib.STEP_PARAMS_WORDS), device=d, dtype=torch.int32)
         self.ctl = torch.zeros((B, _lib.STEP_CTL_WORDS), device=d, dtype=torch.int32)
-        self.rew_xref = float(getattr(env, "rew_xref", 0.0))
         self.graph = None
         self._plan_c = self._make_plan()
 
