@@ -251,6 +251,40 @@ int mbd_bbo_batch_step_launch(const mbd_step_plan* plan, int B, int Ndiffuse, in
 /* sizeof / offsetof of mbd_bbo_bufs and the MBD_BBO_* values (cross-checked against the ctypes mirror) */
 int mbd_bbo_abi_sizes(int32_t* out, int n);
 
+/* ---- model-based diffusion over the weights of a 784-32-32-10 MLP (upstream mbd/blackbox/mbd_mnist.py) ---------------------
+ * One solve (B = 1) laid out as mbd_batch_step_launch with H = 1 and nu = 26506 (the parameter row of csrc/mnist.cuh: W1
+ * transposed, b1, W2, b2, W3, b3).  A step is six parameterless launches (graph-capturable): sampling of the six tensors with the
+ * keys of keys_dev[i]; the forward pass of all N models on the minibatch batch_idx_dev[i] (layer 1 on the tensor cores, split
+ * TF32) -> rews = Js; the MPPI weights (mbd_pi_batch_step_launch's launch (2)) -> rew_hist[i] = Js.mean(); the weighted mean in
+ * two launches -> Ybars[i - 1]; the accuracy of the new mean on the training and test sets -> acc_hist[i] (every eval_every
+ * steps, others keep what the caller put there).  MBD_EINVAL (with mbd_last_error) before any CUDA call for layer sizes other
+ * than 784-32-32-10, N < 1 or N > n_train, Ndiffuse < 2, missing buffers, a plan with a model / demo / P != 1 / H != 1 /
+ * nu != 26506, or the other plan errors of mbd_batch_step_launch. */
+#define MBD_MNIST_HNU 26506
+typedef struct mbd_mnist_bufs {
+  const uint8_t* train_images_dev;   /* [n_train][784] */
+  const uint8_t* train_labels_dev;   /* [n_train] */
+  const uint8_t* test_images_dev;    /* [n_test][784] */
+  const uint8_t* test_labels_dev;    /* [n_test] */
+  const uint32_t* keys_dev;          /* [Ndiffuse][12][2]: (noise key, mask key) of W1, b1, W2, b2, W3, b3 for every step */
+  const int32_t* batch_idx_dev;      /* [Ndiffuse][N]: the minibatch of every step (mbd_mnist_batch_indices) */
+  int32_t* acc_hist_dev;             /* [Ndiffuse][2]: train / test correct-counts of the mean after step i */
+  int32_t layers[4];                 /* must be {784, 32, 32, 10} */
+  int32_t n_train, n_test, eval_every;
+} mbd_mnist_bufs;
+int mbd_mnist_step_launch(const mbd_step_plan* plan, int Ndiffuse, const mbd_mnist_bufs* bufs, mbd_stream s);
+/* Test entry point: Js[n] of models Y0s_dev [n_models][26506] on the images rows_dev [n_img] of the training set of bufs (no step
+ * counter); z1_dev [n_models][n_img][32] (or NULL) receives the layer-1 pre-activations sum_k x_k W1[k][o] / 255 (before b1). */
+int mbd_mnist_forward(const float* Y0s_dev, int n_models, const mbd_mnist_bufs* bufs, const int32_t* rows_dev, int n_img,
+                      float* Js_dev, float* z1_dev, mbd_stream s);
+/* The minibatch table: row t (1 <= t < Ndiffuse) = permutation(batch_rng_t, n_data)[:N] with two rounds of a stable sort by
+ * random_bits(sub_r, (n_data,)); sub_keys_host [Ndiffuse][2][2] = the two round keys of every step.  scratch_dev NULL: writes the
+ * scratch size needed to *scratch_bytes and returns.  Synchronous on the stream's work only (no host synchronisation). */
+int mbd_mnist_batch_indices(const uint32_t* sub_keys_host, int Ndiffuse, int n_data, int N, int32_t* idx_dev, void* scratch_dev,
+                            size_t* scratch_bytes, mbd_stream s);
+/* sizeof / offsetof of mbd_mnist_bufs and MBD_MNIST_HNU (cross-checked against the ctypes mirror) */
+int mbd_mnist_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

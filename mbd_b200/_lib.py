@@ -55,6 +55,14 @@ class BboBufs(ctypes.Structure):
     _fields_ = [("init_keys_dev", c_vp), ("best_hist_dev", c_vp), ("x_min", ctypes.c_float), ("x_max", ctypes.c_float)]
 
 
+class MnistBufs(ctypes.Structure):
+    """mbd_mnist_bufs (include/mbd_b200.h): what an MNIST step adds to a step plan"""
+    _fields_ = [("train_images_dev", c_vp), ("train_labels_dev", c_vp), ("test_images_dev", c_vp), ("test_labels_dev", c_vp),
+                ("keys_dev", c_vp), ("batch_idx_dev", c_vp), ("acc_hist_dev", c_vp), ("layers", ctypes.c_int32 * 4),
+                ("n_train", ctypes.c_int32), ("n_test", ctypes.c_int32), ("eval_every", ctypes.c_int32)]
+
+
+MNIST_HNU = 26506        # MBD_MNIST_HNU
 BBO_FNS = {"Ackley": 1, "Rastrigin": 2, "Levy": 3}   # MBD_BBO_ACKLEY / MBD_BBO_RASTRIGIN / MBD_BBO_LEVY
 PI_METHODS = {"mppi": 1, "cma-es": 2, "cem": 3}   # MBD_PI_MPPI / MBD_PI_CMAES / MBD_PI_CEM
 PI_IDX_STRIDE = 16       # MBD_PI_IDX_STRIDE: ints per problem in cem_idx (10 picks, then the count)
@@ -114,6 +122,11 @@ def lib():
     L.mbd_bbo_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
                                             ctypes.POINTER(BboBufs), c_vp]
     L.mbd_bbo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_mnist_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.POINTER(MnistBufs), c_vp]
+    L.mbd_mnist_forward.argtypes = [c_vp, ctypes.c_int, ctypes.POINTER(MnistBufs), c_vp, ctypes.c_int, c_vp, c_vp, c_vp]
+    L.mbd_mnist_batch_indices.argtypes = [c_u32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp, c_vp,
+                                          ctypes.POINTER(ctypes.c_size_t), c_vp]
+    L.mbd_mnist_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes = [ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -128,7 +141,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_model_set_group_map", "mbd_set_group_stagger", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

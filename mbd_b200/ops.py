@@ -233,6 +233,34 @@ def bbo_batch_step_launch(plan: "_lib.StepPlan", B: int, Ndiffuse: int, fn: int,
                                                _stream()), "mbd_bbo_batch_step_launch")
 
 
+def mnist_step_launch(plan: "_lib.StepPlan", Ndiffuse: int, bufs: "_lib.MnistBufs"):
+    """one MNIST diffusion step (mbd_mnist_step_launch): six launches, parameters read from device tables"""
+    check(_lib.lib().mbd_mnist_step_launch(ctypes.byref(plan), int(Ndiffuse), ctypes.byref(bufs), _stream()), "mbd_mnist_step_launch")
+
+
+def mnist_forward(Y0s: torch.Tensor, bufs: "_lib.MnistBufs", rows: torch.Tensor, Js_out: torch.Tensor, z1_out: Optional[torch.Tensor] = None):
+    """Js [n] of the parameter rows Y0s [n, 26506] on the training images `rows` [n_img] (int32); z1_out [n, n_img, 32] optional"""
+    _dev(Y0s), _dev(rows, torch.int32), _dev(Js_out)
+    if z1_out is not None:
+        _dev(z1_out)
+    check(_lib.lib().mbd_mnist_forward(_p(Y0s), int(Y0s.shape[0]), ctypes.byref(bufs), _p(rows), int(rows.numel()), _p(Js_out),
+                                       _p(z1_out), _stream()), "mbd_mnist_forward")
+
+
+def mnist_batch_indices(sub_keys: np.ndarray, Ndiffuse: int, n_data: int, N: int, idx_out: torch.Tensor):
+    """the minibatch table [Ndiffuse, N] of a solve from the permutation round keys sub_keys [Ndiffuse, 2, 2] (uint32)"""
+    _dev(idx_out, torch.int32)
+    k = np.ascontiguousarray(sub_keys, dtype=np.uint32)
+    L = _lib.lib()
+    nbytes = ctypes.c_size_t(0)
+    check(L.mbd_mnist_batch_indices(k.ctypes.data_as(_lib.c_u32p), int(Ndiffuse), int(n_data), int(N), None, None,
+                                    ctypes.byref(nbytes), _stream()), "mbd_mnist_batch_indices")
+    scratch = torch.empty(int(nbytes.value), device=idx_out.device, dtype=torch.uint8)
+    check(L.mbd_mnist_batch_indices(k.ctypes.data_as(_lib.c_u32p), int(Ndiffuse), int(n_data), int(N), _p(idx_out), _p(scratch),
+                                    ctypes.byref(nbytes), _stream()), "mbd_mnist_batch_indices")
+    torch.cuda.current_stream().synchronize()   # the scratch is freed on return
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""
