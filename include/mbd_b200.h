@@ -285,6 +285,63 @@ int mbd_mnist_batch_indices(const uint32_t* sub_keys_host, int Ndiffuse, int n_d
 /* sizeof / offsetof of mbd_mnist_bufs and MBD_MNIST_HNU (cross-checked against the ctypes mirror) */
 int mbd_mnist_abi_sizes(int32_t* out, int n);
 
+/* ---- a batch of environments stepped together on the device (vmap(env.reset) / vmap(env.step) with Brax's training wrappers) --
+ * B environments of one kind, each with its own state, stepped by two launches: (1) the env's rollout kernel with H = 1 and a
+ * per-sample start state (state -> next_state, reward), (2) one thread per env that computes the observation (xpbd envs: com.to_world
+ * and kinematics.inverse in float64 from the float32 state, rounded once: include/mbd_kin64.h), the env's done, the episode counters
+ * and the auto-reset, and writes the chosen state back into state.  Both launches read everything from the plan, allocate nothing
+ * and do not synchronise: a step can be captured in a CUDA graph.  Buffers (device, caller-owned, fixed for the plan's lifetime):
+ *   state / next_state / first_state [B][S] (S = Lsim * 13, pushT 16, car2d 3), actions [B][Nu], obs / first_obs [B][O],
+ *   reward / done / truncation / steps [B] (float32, steps counts env steps since the last reset).
+ * episode_length > 0 adds Brax's EpisodeWrapper + AutoResetWrapper (action_repeat 1): steps is zeroed where the previous done was set,
+ * then steps += 1; done = steps >= episode_length ? 1 : env_done; truncation = steps >= episode_length ? 1 - env_done : 0; where done
+ * is set, state and obs are replaced by first_state and first_obs (reward and done of the step are returned as computed). */
+enum { MBD_VEC_XPBD = 0, MBD_VEC_CAR2D = 1, MBD_VEC_PUSHT = 2 };
+enum { MBD_VEC_OBS_QQD = 0,     /* q | qd (humanoids, cartpole) */
+       MBD_VEC_OBS_HOPPER = 1,  /* q with q[1] = x.pos[0, 2], clip(qd, -10, 10) (hopper, walker2d) */
+       MBD_VEC_OBS_SKIP2 = 2,   /* q[2:] | qd (ant) */
+       MBD_VEC_OBS_SKIP1 = 3,   /* q[1:] | qd (halfcheetah) */
+       MBD_VEC_OBS_STATE = 4 }; /* the flat state itself (pushT q | qd, car2d x) */
+enum { MBD_VEC_DONE_ZERO = 0, MBD_VEC_DONE_COUNTER = 1 /* humanoidtrack: done = previous done + 1 */, MBD_VEC_DONE_PUSHT = 2 /* reward > 0.95 */ };
+enum { MBD_VEC_RESET_NONE = 0 /* init_q, qd = 0 */, MBD_VEC_RESET_UNIFORM = 1 /* q, qd + U(lo, hi) */,
+       MBD_VEC_RESET_NORMAL = 2 /* q + U(lo, hi), qd = clip(sigma N(0, 1), -1, 1) */, MBD_VEC_RESET_PUSHT = 3, MBD_VEC_RESET_CONST = 4 };
+#define MBD_VEC_MAX_B 65536
+/* reset table (float32, MBD_VEC_RT_* words then init_q [nq] and the q offset [nq]) */
+enum { MBD_VEC_RT_KIND = 0, MBD_VEC_RT_LO = 1, MBD_VEC_RT_HI = 2, MBD_VEC_RT_SIGMA = 3, MBD_VEC_RT_HAS_OFF = 4, MBD_VEC_RT_Q = 8 };
+typedef struct mbd_vec_plan {
+  int32_t kind;                 /* MBD_VEC_* */
+  int32_t B;
+  const mbd_model* model;       /* MBD_VEC_XPBD: the env's model; NULL otherwise */
+  const float* params_dev;      /* car2d / pushT parameter table (as mbd_car2d_rollout / mbd_pusht_rollout); NULL for xpbd */
+  const double* kin_dev;        /* xpbd: the float64 kinematics table of include/mbd_kin64.h */
+  const float* reset_dev;       /* reset table (MBD_VEC_RT_*) */
+  int32_t obs_layout;           /* MBD_VEC_OBS_* */
+  int32_t done_rule;            /* MBD_VEC_DONE_* */
+  int32_t episode_length;       /* 0 = no episode wrapper / auto-reset */
+  int32_t nq, nqd, nu;          /* joint coordinate / velocity / action sizes (flat envs: state size, 0, nu) */
+  float* state_dev;
+  float* next_state_dev;
+  float* first_state_dev;
+  float* actions_dev;
+  float* obs_dev;
+  float* first_obs_dev;
+  float* reward_dev;
+  float* done_dev;
+  float* truncation_dev;
+  float* steps_dev;
+} mbd_vec_plan;
+/* env.reset(keys[b]) for every env b (keys_dev [B][2] uint32), in the threefry layout of mbd_set_prng_layout: state, first_state, obs,
+ * first_obs, reward (0, pushT its reward), done, truncation 0, steps 0. */
+int mbd_vec_reset(const mbd_vec_plan* plan, const uint32_t* keys_dev, mbd_stream s);
+/* one env step of every env with the actions in plan->actions_dev (launches (1) and (2) above) */
+int mbd_vec_step(const mbd_vec_plan* plan, mbd_stream s);
+/* obs of the states the caller wrote into state_dev; first_state = state, first_obs = obs; reward, done, truncation, steps 0 */
+int mbd_vec_set_state(const mbd_vec_plan* plan, mbd_stream s);
+/* xpbd envs: world link poses x.pos [B][L][3], x.rot [B][L][4] of the current states (PipelineEnv._make_pipeline_state) */
+int mbd_vec_world_poses(const mbd_vec_plan* plan, float* pos_dev, float* rot_dev, mbd_stream s);
+/* sizeof / offsetof of mbd_vec_plan and MBD_K64_WORDS (cross-checked against the ctypes mirror) */
+int mbd_vec_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

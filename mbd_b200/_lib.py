@@ -62,6 +62,23 @@ class MnistBufs(ctypes.Structure):
                 ("n_train", ctypes.c_int32), ("n_test", ctypes.c_int32), ("eval_every", ctypes.c_int32)]
 
 
+class VecPlan(ctypes.Structure):
+    """mbd_vec_plan (include/mbd_b200.h): a batch of envs stepped together on the device"""
+    _fields_ = [("kind", ctypes.c_int32), ("B", ctypes.c_int32), ("model", c_vp), ("params_dev", c_vp), ("kin_dev", c_vp),
+                ("reset_dev", c_vp), ("obs_layout", ctypes.c_int32), ("done_rule", ctypes.c_int32), ("episode_length", ctypes.c_int32),
+                ("nq", ctypes.c_int32), ("nqd", ctypes.c_int32), ("nu", ctypes.c_int32),
+                ("state_dev", c_vp), ("next_state_dev", c_vp), ("first_state_dev", c_vp), ("actions_dev", c_vp), ("obs_dev", c_vp),
+                ("first_obs_dev", c_vp), ("reward_dev", c_vp), ("done_dev", c_vp), ("truncation_dev", c_vp), ("steps_dev", c_vp)]
+
+
+VEC_XPBD, VEC_CAR2D, VEC_PUSHT = 0, 1, 2                                   # MBD_VEC_*
+VEC_OBS = {"qqd": 0, "hopper": 1, "skip2": 2, "skip1": 3, "state": 4}     # MBD_VEC_OBS_*
+VEC_DONE_ZERO, VEC_DONE_COUNTER, VEC_DONE_PUSHT = 0, 1, 2                 # MBD_VEC_DONE_*
+VEC_RESET = {"none": 0, "uniform": 1, "normal": 2, "pusht": 3, "const": 4}  # MBD_VEC_RESET_*
+VEC_RT_Q = 8             # MBD_VEC_RT_Q: first init_q word of the reset table
+VEC_MAX_B = 65536        # MBD_VEC_MAX_B
+K64_WORDS = 920          # MBD_K64_WORDS (include/mbd_kin64.h)
+
 MNIST_HNU = 26506        # MBD_MNIST_HNU
 BBO_FNS = {"Ackley": 1, "Rastrigin": 2, "Levy": 3}   # MBD_BBO_ACKLEY / MBD_BBO_RASTRIGIN / MBD_BBO_LEVY
 PI_METHODS = {"mppi": 1, "cma-es": 2, "cem": 3}   # MBD_PI_MPPI / MBD_PI_CMAES / MBD_PI_CEM
@@ -127,6 +144,11 @@ def lib():
     L.mbd_mnist_batch_indices.argtypes = [c_u32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp, c_vp,
                                           ctypes.POINTER(ctypes.c_size_t), c_vp]
     L.mbd_mnist_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_vec_reset.argtypes = [ctypes.POINTER(VecPlan), c_vp, c_vp]
+    L.mbd_vec_step.argtypes = [ctypes.POINTER(VecPlan), c_vp]
+    L.mbd_vec_set_state.argtypes = [ctypes.POINTER(VecPlan), c_vp]
+    L.mbd_vec_world_poses.argtypes = [ctypes.POINTER(VecPlan), c_vp, c_vp, c_vp]
+    L.mbd_vec_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes = [ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -141,7 +163,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_model_set_group_map", "mbd_set_group_stagger", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

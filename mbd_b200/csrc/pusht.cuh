@@ -270,7 +270,9 @@ __device__ __forceinline__ float pusht_reward(const float* q) {
 }
 
 // sample_elem: the planner's per-element sampler (defined in mbd_b200.cu before this header is included)
-__global__ void __launch_bounds__(64) k_pusht(PushTArgs a) {
+// PS: sample i starts from its own x0 + 16 i (the vector env's step, k_pusht_ps)
+template <bool PS>
+__device__ __forceinline__ void pusht_body(const PushTArgs& a) {
   __shared__ float P[MBD_PT_NPARAM];
   for (int k = threadIdx.x; k < MBD_PT_NPARAM; k += blockDim.x) P[k] = a.params[k];
   __syncthreads();
@@ -286,7 +288,8 @@ __global__ void __launch_bounds__(64) k_pusht(PushTArgs a) {
     ck0 = pb.sp[si].key[0]; ck1 = pb.sp[si].key[1]; csigma = pb.sp[si].sigma; cYbar = pb.Ybars + (size_t)si * HNu;
   }
   float q[MBD_PT_NQ], qd[MBD_PT_NQ];
-  for (int k = 0; k < MBD_PT_NQ; ++k) { q[k] = pb.state_init[k]; qd[k] = pb.state_init[MBD_PT_NQ + k]; }
+  const float* x0 = pb.state_init + (PS ? (size_t)i * MBD_PT_STATE : 0);
+  for (int k = 0; k < MBD_PT_NQ; ++k) { q[k] = x0[k]; qd[k] = x0[MBD_PT_NQ + k]; }
   float sum = 0.0f;
   for (int t = 0; t < a.H; ++t) {
     float* ur = pb.Y0s + ((size_t)i * a.H + t) * 2;
@@ -313,5 +316,7 @@ __global__ void __launch_bounds__(64) k_pusht(PushTArgs a) {
   if (a.final_state)
     for (int k = 0; k < MBD_PT_NQ; ++k) { a.final_state[(size_t)i * MBD_PT_STATE + k] = q[k]; a.final_state[(size_t)i * MBD_PT_STATE + MBD_PT_NQ + k] = qd[k]; }
 }
+__global__ void __launch_bounds__(64) k_pusht(PushTArgs a) { pusht_body<false>(a); }
+__global__ void __launch_bounds__(64) k_pusht_ps(PushTArgs a) { pusht_body<true>(a); }
 
 }  // namespace mbd

@@ -261,6 +261,26 @@ def mnist_batch_indices(sub_keys: np.ndarray, Ndiffuse: int, n_data: int, N: int
     torch.cuda.current_stream().synchronize()   # the scratch is freed on return
 
 
+def vec_reset(plan: "_lib.VecPlan", keys: torch.Tensor):
+    """env.reset(keys[b]) of every env of a vector-env plan (mbd_vec_reset); keys [B, 2] int32 / uint32 bits on the device"""
+    check(_lib.lib().mbd_vec_reset(ctypes.byref(plan), _p(_dev(keys, torch.int32)), _stream()), "mbd_vec_reset")
+
+
+def vec_step(plan: "_lib.VecPlan"):
+    """one env step of every env with the actions in the plan's buffer (mbd_vec_step: two launches, graph-capturable)"""
+    check(_lib.lib().mbd_vec_step(ctypes.byref(plan), _stream()), "mbd_vec_step")
+
+
+def vec_set_state(plan: "_lib.VecPlan"):
+    """observations of the states written into the plan's state buffer; they become the envs' first states (mbd_vec_set_state)"""
+    check(_lib.lib().mbd_vec_set_state(ctypes.byref(plan), _stream()), "mbd_vec_set_state")
+
+
+def vec_world_poses(plan: "_lib.VecPlan", pos: torch.Tensor, rot: torch.Tensor):
+    """x.pos [B, L, 3] and x.rot [B, L, 4] of the current states of an xpbd vector env (mbd_vec_world_poses)"""
+    check(_lib.lib().mbd_vec_world_poses(ctypes.byref(plan), _p(_dev(pos)), _p(_dev(rot)), _stream()), "mbd_vec_world_poses")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""
