@@ -342,6 +342,69 @@ int mbd_vec_world_poses(const mbd_vec_plan* plan, float* pos_dev, float* rot_dev
 /* sizeof / offsetof of mbd_vec_plan and MBD_K64_WORDS (cross-checked against the ctypes mirror) */
 int mbd_vec_abi_sizes(int32_t* out, int n);
 
+/* ---- PPO on the vector env (Brax's ppo.train, v0.10.x line [brax-recalled]; mbd_b200/rl) ---------------------------------------
+ * The acting step, the observation statistics and GAE on the device; the nets, the loss and Adam stay in torch.  A training step's
+ * rollout is one time series of `slots` = U * T acting slots of B envs: obs [slots + 1][B][O], raw [slots][B][Nu], logp / reward /
+ * disc / trunc [slots][B]; trajectory n = u * B + b is slots u * T ... u * T + T - 1 of env b and its bootstrap observation is slot
+ * u * T + T.  act_ctl_dev [4] = {slot t, key row k, ticket (0), 0}: every act launch reads them, and its last CTA advances them.
+ * MBD_EINVAL (with mbd_last_error) before any CUDA call for O outside 1..128, Nu outside 1..32, B outside 1..MBD_VEC_MAX_B or a
+ * missing buffer of the entry point. */
+enum { MBD_PPO_ACT = 0,          /* obs[t] = env obs; reward / disc / trunc [t - 1] = the env's (t > 0); raw[t], logp[t]; actions = tanh(raw)
+                                  * with eps = normal(act_keys[k], (B, Nu)); t += 1, k += 1 */
+       MBD_PPO_RECORD = 1,       /* the records of MBD_PPO_ACT without acting (after an unroll's last step); t = 0 */
+       MBD_PPO_EVAL = 2,         /* t > 0: ret += active * reward, active *= 1 - done; then act as MBD_PPO_ACT without records; t += 1, k += 1 */
+       MBD_PPO_EVAL_RECORD = 3 };/* the accumulation of MBD_PPO_EVAL without acting; t = 0 */
+#define MBD_PPO_MAX_OBS 128
+#define MBD_PPO_MAX_NU 32
+#define MBD_PPO_MAX_MB 4096     /* trajectories per minibatch; a GAE thread takes every 1024th */
+#define MBD_PPO_STAT_ROWS 256    /* rows per partial sum of mbd_ppo_obs_stats */
+typedef struct mbd_ppo_plan {
+  int32_t B, O, nu;              /* envs, observation size, action size */
+  int32_t slots;                 /* acting slots of one training step (U * T) */
+  int32_t unroll;                /* T */
+  int32_t mb;                    /* trajectories per minibatch (GAE) */
+  float reward_scaling, discount, gae_lambda;
+  int32_t act_key_rows;          /* rows of act_keys_dev: an act launch past the table writes nothing */
+  int32_t loss_key_rows;         /* rows of loss_keys_dev: a GAE launch past the table draws no noise */
+  const float* policy_dev;       /* flat policy parameters (include/mbd_ppo.h) */
+  const float* mean_dev;         /* [O] running mean (float32) */
+  const float* std_dev;          /* [O] running std (float32) */
+  const uint32_t* act_keys_dev;  /* [n][2] act keys, row k */
+  int32_t* act_ctl_dev;          /* [4] */
+  const float* env_obs_dev;      /* the vector env's obs [B][O], reward, done, truncation [B] and actions [B][Nu] */
+  const float* env_reward_dev;
+  const float* env_done_dev;
+  const float* env_trunc_dev;
+  float* env_actions_dev;
+  float* obs_dev;                /* the rollout (MBD_PPO_ACT / MBD_PPO_RECORD, and GAE) */
+  float* raw_dev;
+  float* logp_dev;
+  float* reward_dev;
+  float* disc_dev;
+  float* trunc_dev;
+  float* ret_dev;                /* evaluation: [B] episode return and active flag */
+  float* active_dev;
+  double* stat_dev;              /* [1 + 2 O]: count, mean, summed variance (float64) */
+  double* stat_scratch_dev;      /* [ceil(slots * B / MBD_PPO_STAT_ROWS)][2][O] */
+  const uint32_t* loss_keys_dev; /* [n][2] loss keys, row *loss_ctl_dev */
+  const int32_t* loss_ctl_dev;
+  const int32_t* traj_dev;       /* [mb] trajectory ids of the minibatch */
+  const float* values_dev;       /* [T + 1][mb] values of the minibatch's observations (row T: the bootstrap values) */
+  float* vs_dev;                 /* [T][mb] value targets */
+  float* adv_dev;                /* [T][mb] normalised advantages */
+  float* ent_eps_dev;            /* [T][mb][Nu] = normal(loss key, (T, mb, Nu)) */
+} mbd_ppo_plan;
+/* one launch: the policy of every env (warp per env, lane per hidden unit) in the given MBD_PPO_* mode */
+int mbd_ppo_act(const mbd_ppo_plan* plan, int mode, mbd_stream s);
+/* running_statistics.update with obs rows 0 .. slots * B - 1 (two launches, float64 sums in a fixed order); writes mean_dev / std_dev
+ * (std = clip(sqrt(summed_var / count), 1e-6, 1e6)) */
+int mbd_ppo_obs_stats(const mbd_ppo_plan* plan, mbd_stream s);
+/* one launch per minibatch: compute_gae with the truncation mask on the trajectories traj_dev (rewards * reward_scaling), the
+ * advantage normalisation (adv - mean) / (std + 1e-8) (population std) and the entropy noise */
+int mbd_ppo_gae(const mbd_ppo_plan* plan, mbd_stream s);
+/* sizeof / offsetof of mbd_ppo_plan and the MBD_PPO_* limits (cross-checked against the ctypes mirror) */
+int mbd_ppo_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

@@ -71,6 +71,22 @@ class VecPlan(ctypes.Structure):
                 ("first_obs_dev", c_vp), ("reward_dev", c_vp), ("done_dev", c_vp), ("truncation_dev", c_vp), ("steps_dev", c_vp)]
 
 
+class PpoPlan(ctypes.Structure):
+    """mbd_ppo_plan (include/mbd_b200.h): the PPO acting step, observation statistics and GAE"""
+    _fields_ = [("B", ctypes.c_int32), ("O", ctypes.c_int32), ("nu", ctypes.c_int32), ("slots", ctypes.c_int32),
+                ("unroll", ctypes.c_int32), ("mb", ctypes.c_int32), ("reward_scaling", ctypes.c_float), ("discount", ctypes.c_float),
+                ("gae_lambda", ctypes.c_float), ("act_key_rows", ctypes.c_int32), ("loss_key_rows", ctypes.c_int32),
+                ("policy_dev", c_vp), ("mean_dev", c_vp), ("std_dev", c_vp), ("act_keys_dev", c_vp), ("act_ctl_dev", c_vp),
+                ("env_obs_dev", c_vp), ("env_reward_dev", c_vp), ("env_done_dev", c_vp), ("env_trunc_dev", c_vp),
+                ("env_actions_dev", c_vp), ("obs_dev", c_vp), ("raw_dev", c_vp), ("logp_dev", c_vp), ("reward_dev", c_vp),
+                ("disc_dev", c_vp), ("trunc_dev", c_vp), ("ret_dev", c_vp), ("active_dev", c_vp), ("stat_dev", c_vp),
+                ("stat_scratch_dev", c_vp), ("loss_keys_dev", c_vp), ("loss_ctl_dev", c_vp), ("traj_dev", c_vp), ("values_dev", c_vp),
+                ("vs_dev", c_vp), ("adv_dev", c_vp), ("ent_eps_dev", c_vp)]
+
+
+PPO_ACT, PPO_RECORD, PPO_EVAL, PPO_EVAL_RECORD = 0, 1, 2, 3   # MBD_PPO_*
+PPO_MAX_OBS, PPO_MAX_NU, PPO_MAX_MB, PPO_STAT_ROWS = 128, 32, 4096, 256
+
 VEC_XPBD, VEC_CAR2D, VEC_PUSHT = 0, 1, 2                                   # MBD_VEC_*
 VEC_OBS = {"qqd": 0, "hopper": 1, "skip2": 2, "skip1": 3, "state": 4}     # MBD_VEC_OBS_*
 VEC_DONE_ZERO, VEC_DONE_COUNTER, VEC_DONE_PUSHT = 0, 1, 2                 # MBD_VEC_DONE_*
@@ -149,6 +165,10 @@ def lib():
     L.mbd_vec_set_state.argtypes = [ctypes.POINTER(VecPlan), c_vp]
     L.mbd_vec_world_poses.argtypes = [ctypes.POINTER(VecPlan), c_vp, c_vp, c_vp]
     L.mbd_vec_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_ppo_act.argtypes = [ctypes.POINTER(PpoPlan), ctypes.c_int, c_vp]
+    L.mbd_ppo_obs_stats.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
+    L.mbd_ppo_gae.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
+    L.mbd_ppo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes = [ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -163,7 +183,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_model_set_group_map", "mbd_set_group_stagger", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

@@ -281,6 +281,21 @@ def vec_world_poses(plan: "_lib.VecPlan", pos: torch.Tensor, rot: torch.Tensor):
     check(_lib.lib().mbd_vec_world_poses(ctypes.byref(plan), _p(_dev(pos)), _p(_dev(rot)), _stream()), "mbd_vec_world_poses")
 
 
+def ppo_act(plan: "_lib.PpoPlan", mode: int):
+    """one PPO acting launch (mbd_ppo_act) in mode _lib.PPO_*: the policy of every env, its records or the evaluation return"""
+    check(_lib.lib().mbd_ppo_act(ctypes.byref(plan), int(mode), _stream()), "mbd_ppo_act")
+
+
+def ppo_obs_stats(plan: "_lib.PpoPlan"):
+    """running_statistics.update with the rollout's acting observations (mbd_ppo_obs_stats: two launches)"""
+    check(_lib.lib().mbd_ppo_obs_stats(ctypes.byref(plan), _stream()), "mbd_ppo_obs_stats")
+
+
+def ppo_gae(plan: "_lib.PpoPlan"):
+    """GAE, the advantage normalisation and the entropy noise of one minibatch (mbd_ppo_gae: one launch)"""
+    check(_lib.lib().mbd_ppo_gae(ctypes.byref(plan), _stream()), "mbd_ppo_gae")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""
