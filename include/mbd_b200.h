@@ -405,6 +405,56 @@ int mbd_ppo_gae(const mbd_ppo_plan* plan, mbd_stream s);
 /* sizeof / offsetof of mbd_ppo_plan and the MBD_PPO_* limits (cross-checked against the ctypes mirror) */
 int mbd_ppo_abi_sizes(int32_t* out, int n);
 
+/* ---- SAC on the vector env (Brax's sac.train, v0.10.x line [brax-recalled]; mbd_b200/rl/sac.py) ---------------------------------
+ * The acting step, the replay ring and its uniform sampler on the device; the losses and the three Adam optimisers stay in torch.
+ * The ring holds `capacity` rows of include/mbd_sac.h's layout; ring_ctl_dev [4] = {pos (next write row), size, ticket (0), 0} gives
+ * Brax's queue: logical row i (oldest first) is physical row (pos - size + i) mod capacity.  act_ctl_dev [4] is PPO's {step t, key
+ * row k, ticket (0), 0}; sample_ctl_dev [4] = {training step s, ticket (0), buffer key word 0, word 1}.  Each launch's last CTA
+ * advances its control words, so a training step is graph-capturable.  MBD_EINVAL (with mbd_last_error) before any CUDA call for O
+ * outside 1..128, Nu outside 1..32, B outside 1..MBD_VEC_MAX_B, capacity outside B..MBD_SAC_MAX_CAPACITY or a missing buffer. */
+enum { MBD_SAC_ACT = 0,          /* actions = tanh(raw), eps = normal(act_keys[k], (B, Nu)); obs and action into ring rows pos + b, obs
+                                  * into stage_obs; k += 1 */
+       MBD_SAC_EVAL = 1,         /* PPO's MBD_PPO_EVAL: t > 0: ret += active * reward, active *= 1 - done; then act without records */
+       MBD_SAC_EVAL_RECORD = 2 };/* the accumulation of MBD_SAC_EVAL without acting; t = 0 */
+#define MBD_SAC_MAX_CAPACITY (1 << 24)
+typedef struct mbd_sac_plan {
+  int32_t B, O, nu;              /* envs, observation size, action size */
+  int32_t capacity;              /* ring rows (max_replay_size) */
+  int32_t batch;                 /* rows per gradient update (batch_size) */
+  int32_t updates;               /* gradient updates per training step (grad_updates_per_step) */
+  int32_t act_key_rows;          /* rows of act_keys_dev: an act launch past the table writes nothing */
+  int32_t noise_key_rows;        /* training steps of noise_keys_dev: a sample launch past the table writes nothing */
+  const float* policy_dev;       /* flat policy parameters (include/mbd_sac.h) */
+  const float* mean_dev;         /* [O] running mean (float32) */
+  const float* std_dev;          /* [O] running std (float32) */
+  const uint32_t* act_keys_dev;  /* [n][2] act keys, row k */
+  int32_t* act_ctl_dev;          /* [4] */
+  const float* env_obs_dev;      /* the vector env's obs [B][O], reward, done, truncation [B] and actions [B][Nu] */
+  const float* env_reward_dev;
+  const float* env_done_dev;
+  const float* env_trunc_dev;
+  float* env_actions_dev;
+  float* ret_dev;                /* evaluation: [B] episode return and active flag */
+  float* active_dev;
+  float* stage_obs_dev;          /* [B][O] the acting observations (the statistics' input) */
+  float* ring_dev;               /* [capacity][mbd_sac_row(O, Nu)] */
+  int32_t* ring_ctl_dev;         /* [4] */
+  int32_t* sample_ctl_dev;       /* [4] */
+  const uint32_t* noise_keys_dev;/* [noise_key_rows][updates][3][2]: key_alpha, key_critic, key_actor of every update */
+  int32_t* idx_dev;              /* [updates * batch] logical indices of the sample */
+  float* batch_dev;              /* [updates][batch][row] the gathered rows */
+  float* eps_dev;                /* [3][updates][batch][Nu] = normal(key_{alpha, critic, actor}, (batch, Nu)) of every update */
+} mbd_sac_plan;
+/* one launch: the policy of every env (CTA = a tile of envs, thread = hidden unit) in the given MBD_SAC_* mode */
+int mbd_sac_act(const mbd_sac_plan* plan, int mode, mbd_stream s);
+/* one launch after mbd_vec_step: reward, 1 - done, next obs and truncation into ring rows pos + b; pos += B, size = min(size + B, cap) */
+int mbd_sac_record(const mbd_sac_plan* plan, mbd_stream s);
+/* one launch per training step: buffer key, sample key = split(buffer key); updates * batch randint indices in 0 .. size - 1 from
+ * sample key, the gathered rows, and the three noise tensors of every update from noise_keys row s; s += 1 */
+int mbd_sac_sample(const mbd_sac_plan* plan, mbd_stream s);
+/* sizeof / offsetof of mbd_sac_plan and the MBD_SAC_* limits (cross-checked against the ctypes mirror) */
+int mbd_sac_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

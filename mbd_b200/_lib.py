@@ -84,8 +84,21 @@ class PpoPlan(ctypes.Structure):
                 ("vs_dev", c_vp), ("adv_dev", c_vp), ("ent_eps_dev", c_vp)]
 
 
+class SacPlan(ctypes.Structure):
+    """mbd_sac_plan (include/mbd_b200.h): the SAC acting step, the replay record and the replay sampler"""
+    _fields_ = [("B", ctypes.c_int32), ("O", ctypes.c_int32), ("nu", ctypes.c_int32), ("capacity", ctypes.c_int32),
+                ("batch", ctypes.c_int32), ("updates", ctypes.c_int32), ("act_key_rows", ctypes.c_int32), ("noise_key_rows", ctypes.c_int32),
+                ("policy_dev", c_vp), ("mean_dev", c_vp), ("std_dev", c_vp), ("act_keys_dev", c_vp), ("act_ctl_dev", c_vp),
+                ("env_obs_dev", c_vp), ("env_reward_dev", c_vp), ("env_done_dev", c_vp), ("env_trunc_dev", c_vp),
+                ("env_actions_dev", c_vp), ("ret_dev", c_vp), ("active_dev", c_vp), ("stage_obs_dev", c_vp), ("ring_dev", c_vp),
+                ("ring_ctl_dev", c_vp), ("sample_ctl_dev", c_vp), ("noise_keys_dev", c_vp), ("idx_dev", c_vp), ("batch_dev", c_vp),
+                ("eps_dev", c_vp)]
+
+
 PPO_ACT, PPO_RECORD, PPO_EVAL, PPO_EVAL_RECORD = 0, 1, 2, 3   # MBD_PPO_*
 PPO_MAX_OBS, PPO_MAX_NU, PPO_MAX_MB, PPO_STAT_ROWS = 128, 32, 4096, 256
+SAC_ACT, SAC_EVAL, SAC_EVAL_RECORD = 0, 1, 2                   # MBD_SAC_*
+SAC_MAX_CAPACITY, SAC_HIDDEN = 1 << 24, 256
 
 VEC_XPBD, VEC_CAR2D, VEC_PUSHT = 0, 1, 2                                   # MBD_VEC_*
 VEC_OBS = {"qqd": 0, "hopper": 1, "skip2": 2, "skip1": 3, "state": 4}     # MBD_VEC_OBS_*
@@ -169,6 +182,10 @@ def lib():
     L.mbd_ppo_obs_stats.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
     L.mbd_ppo_gae.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
     L.mbd_ppo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_sac_act.argtypes = [ctypes.POINTER(SacPlan), ctypes.c_int, c_vp]
+    L.mbd_sac_record.argtypes = [ctypes.POINTER(SacPlan), c_vp]
+    L.mbd_sac_sample.argtypes = [ctypes.POINTER(SacPlan), c_vp]
+    L.mbd_sac_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes = [ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -183,7 +200,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_model_set_group_map", "mbd_set_group_stagger", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_sample_rollout", "mbd_reverse_step", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_peer_gather", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

@@ -296,6 +296,22 @@ def ppo_gae(plan: "_lib.PpoPlan"):
     check(_lib.lib().mbd_ppo_gae(ctypes.byref(plan), _stream()), "mbd_ppo_gae")
 
 
+def sac_act(plan: "_lib.SacPlan", mode: int):
+    """one SAC acting launch (mbd_sac_act) in mode _lib.SAC_*: the policy of every env and its half of the replay rows, or the
+    evaluation return"""
+    check(_lib.lib().mbd_sac_act(ctypes.byref(plan), int(mode), _stream()), "mbd_sac_act")
+
+
+def sac_record(plan: "_lib.SacPlan"):
+    """the env step's reward, discount, next obs and truncation into the replay rows, and the ring's advance (mbd_sac_record)"""
+    check(_lib.lib().mbd_sac_record(ctypes.byref(plan), _stream()), "mbd_sac_record")
+
+
+def sac_sample(plan: "_lib.SacPlan"):
+    """one training step's replay sample: indices, gathered rows and the three noise tensors of every update (mbd_sac_sample)"""
+    check(_lib.lib().mbd_sac_sample(ctypes.byref(plan), _stream()), "mbd_sac_sample")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

@@ -99,3 +99,61 @@ def entropy(logits: torch.Tensor, eps: torch.Tensor) -> torch.Tensor:
     scale = F.softplus(s) + MIN_STD
     ent = 0.5 + (HALF_LOG_2PI + torch.log(scale))
     return (ent + tanh_log_det_jacobian(eps * scale + loc)).sum(-1)
+
+
+# ---- SAC (brax.training.agents.sac.networks **[brax-recalled]**) -------------------------------------------------------------------
+# policy: O -> 256 -> 256 -> 2 Nu, ReLU between layers, the layout above (include/mbd_sac.h reads it); Q: two critics, each
+# concat(normalize(obs), action) -> 256 -> 256 -> 1 with ReLU.  The Q buffer is layer-major so that both critics run as one batched
+# matmul: W_l [2][in][out], then b_l [2][out], layer by layer.  Init: critic c takes key c of split(key_q) and draws as init_params.
+SAC_HIDDEN = (256, 256)
+N_CRITICS = 2
+
+
+def sac_policy_sizes(O: int, nu: int):
+    return layer_sizes(O, 2 * nu, SAC_HIDDEN)
+
+
+def sac_q_sizes(O: int, nu: int):
+    """the sizes of one critic"""
+    return layer_sizes(O + nu, 1, SAC_HIDDEN)
+
+
+def sac_q_num_params(O: int, nu: int) -> int:
+    return N_CRITICS * num_params(sac_q_sizes(O, nu))
+
+
+def sac_q_unflatten(flat, sizes):
+    """[(W [2, in, out], b [2, 1, out])] views of a layer-major Q buffer"""
+    out, k = [], 0
+    for i, o in sizes:
+        W = flat[k:k + N_CRITICS * i * o].reshape(N_CRITICS, i, o)
+        k += N_CRITICS * i * o
+        out.append((W, flat[k:k + N_CRITICS * o].reshape(N_CRITICS, 1, o)))
+        k += N_CRITICS * o
+    if k != len(flat):
+        raise ValueError(f"flat buffer has {len(flat)} floats, the layout {k}")
+    return out
+
+
+def sac_q_init(key, sizes) -> np.ndarray:
+    critics = [unflatten(init_params(k, sizes), sizes) for k in prng.split(key, N_CRITICS)]
+    return np.concatenate([np.concatenate([np.stack([np.asarray(c[l][0]) for c in critics]).ravel(),
+                                           np.stack([np.asarray(c[l][1]) for c in critics]).ravel()]) for l in range(len(sizes))])
+
+
+def relu_mlp(x: torch.Tensor, layers) -> torch.Tensor:
+    for l, (W, b) in enumerate(layers):
+        x = torch.addmm(b, x, W)
+        if l + 1 < len(layers):
+            x = F.relu(x)
+    return x
+
+
+def sac_q(layers, x: torch.Tensor, action: torch.Tensor) -> torch.Tensor:
+    """Q values [2, n] of both critics at (normalised obs x [n, O], action [n, Nu])"""
+    h = torch.cat([x, action], -1).unsqueeze(0).expand(N_CRITICS, -1, -1)
+    for l, (W, b) in enumerate(layers):
+        h = torch.baddbmm(b, h, W)
+        if l + 1 < len(layers):
+            h = F.relu(h)
+    return h.squeeze(-1)

@@ -1,0 +1,453 @@
+"""SAC (Brax's `brax.training.agents.sac.train`, v0.10.x line **[brax-recalled]**) on the device vector env.
+
+Acting is one CUDA launch per env step (`mbd_sac_act`, csrc/sac.cuh) followed by the two launches of the vector env's step, the
+replay record (`mbd_sac_record`) and PPO's observation statistics (`mbd_ppo_obs_stats` over the B acting observations).  The replay
+buffer is a device ring with Brax's queue semantics, and one `mbd_sac_sample` launch per training step draws the batch of every
+gradient update and the noise of its three losses.  The losses and the three Adam optimisers are torch fp32.  Every key of a run is
+computed on the host up front (`key_chain`) and read on the device through counters: a training step is the acting graph, the
+sampling graph and 64 replays of the update graph, with no host synchronisation.
+
+Step accounting as Brax: num_prefill_actor_steps = ceil(min_replay_size / num_envs); num_evals_after_init = max(num_evals - 1, 1);
+training steps per epoch = ceil((num_timesteps - prefill env steps) / (num_evals_after_init * num_envs)); the reported env-step count
+includes the prefill.  Declared deviations: the initial parameters (networks.py), the float64 observation statistics, the Polyak
+update as target + tau (q - target) (torch's lerp; Brax writes target (1 - tau) + q tau), and the project's fp32 transcendentals.
+"""
+from __future__ import annotations
+
+import dataclasses
+import time
+from typing import Callable, Optional
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from .. import _lib, ops, prng
+from ..envs import get_env
+from ..envs.vec import VecEnv
+from . import networks as nets
+from .ppo import _i32, fold_in
+
+ALPHA_LEARNING_RATE = 3e-4      # Brax's alpha optimiser is adam(3e-4) whatever learning_rate is
+
+
+# ---- step accounting and the key chain (host only) -------------------------------------------------------------------------------
+@dataclasses.dataclass
+class Counts:
+    prefill_steps: int           # num_prefill_actor_steps
+    prefill_env_steps: int
+    num_evals_after_init: int
+    steps_per_epoch: int         # training steps between two evaluations
+    env_steps_per_training_step: int
+
+
+def counts(num_timesteps: int, num_envs: int, min_replay_size: int, num_evals: int) -> Counts:
+    prefill = -(-min_replay_size // num_envs)
+    prefill_env = prefill * num_envs
+    if num_timesteps < prefill_env:
+        raise ValueError("num_timesteps must cover the replay prefill (ceil(min_replay_size / num_envs) * num_envs env steps)")
+    after = max(num_evals - 1, 1)
+    return Counts(prefill, prefill_env, after, -(-(num_timesteps - prefill_env) // (after * num_envs)), num_envs)
+
+
+def split_many(keys, num: int) -> np.ndarray:
+    """prng.split(k, num) of every row of keys [n, 2] at once: [n, num, 2] (the current threefry layout)"""
+    keys = np.ascontiguousarray(keys, np.uint32).reshape(-1, 2)
+    k = (keys[:, 0:1], keys[:, 1:2])
+    idx = np.arange(num, dtype=np.uint32)[None, :]
+    if prng._PARTITIONABLE:
+        o0, o1 = prng.threefry2x32(k, np.zeros_like(idx), idx)
+        return np.stack([o0, o1], -1).astype(np.uint32)
+    o0, o1 = prng.threefry2x32(k, idx, idx + np.uint32(num))      # bits(key, 2 num): blocks (i, i + num)
+    return np.concatenate([o0, o1], 1).reshape(-1, num, 2).astype(np.uint32)
+
+
+@dataclasses.dataclass
+class Keys:
+    policy: np.ndarray           # init keys of the policy and of the two critics
+    q: np.ndarray
+    env: np.ndarray              # [num_envs, 2] reset keys of the training envs
+    buffer: np.ndarray           # [2] the replay buffer's initial key
+    act: np.ndarray              # [prefill_steps + steps, 2] act keys: the prefill steps, then every training step's experience key
+    noise: np.ndarray            # [steps, updates, 3, 2] key_alpha, key_critic, key_actor of every update
+    eval_reset: np.ndarray       # [num_evals_after_init + 1, num_eval_envs, 2]
+    eval_act: np.ndarray         # [num_evals_after_init + 1, episode_length, 2]
+
+
+def key_chain(seed: int, c: Counts, num_envs: int, updates: int, num_eval_envs: int, episode_length: int) -> Keys:
+    """sac.train's keys: PRNGKey(seed) -> global, local; local = fold_in(local, 0); local, rb_key, env_key, eval_key = split(local, 4);
+    policy, q = split(global); the buffer key split(rb_key, 1)[0].  Prefill: `prefill_key, local = split(local)`, k = split(prefill_key,
+    1)[0], per step `k, next = split(k)` and act with k.  Per epoch `epoch_key, local = split(local)`, k = split(epoch_key, 1)[0]; per
+    training step `k, next = split(k)`, `experience_key, training_key = split(k)`; per update `key, key_alpha, key_critic, key_actor =
+    split(key, 4)` from training_key.  The evaluator is PPO's.  The training steps of all epochs and the update chains run as array
+    operations (split_many): a Python loop over the 3.3 M splits of the reference's hopper run takes about a minute."""
+    gk, lk = prng.split(prng.PRNGKey(seed))
+    lk = fold_in(lk, 0)
+    lk, rb_key, env_key, eval_key = prng.split(lk, 4)
+    kp, kq = prng.split(gk)
+    prefill_key, lk = prng.split2(lk)
+    k = prng.split(prefill_key, 1)[0]
+    pre = np.zeros((c.prefill_steps, 2), np.uint32)
+    for i in range(c.prefill_steps):
+        pre[i], k = prng.split2(k)
+    E, S = c.num_evals_after_init, c.steps_per_epoch
+    k = np.zeros((E, 2), np.uint32)
+    for e in range(E):
+        epoch_key, lk = prng.split2(lk)
+        k[e] = prng.split(epoch_key, 1)[0]
+    step = np.zeros((E, S, 2), np.uint32)
+    for s in range(S):
+        kk = split_many(k, 2)
+        step[:, s], k = kk[:, 0], kk[:, 1]
+    et = split_many(step.reshape(-1, 2), 2)
+    key = et[:, 1]
+    noise = np.zeros((E * S, updates, 3, 2), np.uint32)
+    for g in range(updates):
+        k4 = split_many(key, 4)
+        key, noise[:, g] = k4[:, 0], k4[:, 1:]
+    n_eval = E + 1
+    eval_reset = np.zeros((n_eval, num_eval_envs, 2), np.uint32)
+    eval_act = np.zeros((n_eval, episode_length, 2), np.uint32)
+    for i in range(n_eval):
+        eval_key, uk = prng.split2(eval_key)
+        eval_reset[i] = prng.split(uk, num_eval_envs)
+        cur = uk
+        for t in range(episode_length):
+            eval_act[i, t], cur = prng.split2(cur)
+    return Keys(kp, kq, prng.split(env_key, num_envs), prng.split(rb_key, 1)[0], np.concatenate([pre, et[:, 0]]), noise,
+                eval_reset, eval_act)
+
+
+# ---- the learner (torch; runs on any device) --------------------------------------------------------------------------------------
+def unpack_rows(rows: torch.Tensor, O: int, nu: int):
+    """(obs, action, reward, discount, next_obs, truncation) of replay rows [n, 2 O + Nu + 3] (include/mbd_sac.h)"""
+    return (rows[:, :O], rows[:, O:O + nu], rows[:, O + nu], rows[:, O + nu + 1], rows[:, O + nu + 2:2 * O + nu + 2],
+            rows[:, 2 * O + nu + 2])
+
+
+def losses(policy, q, target_q, log_alpha, mean, std, rows, eps, O: int, nu: int, reward_scaling: float, discounting: float):
+    """Brax's alpha, critic and actor losses on one batch: eps [3, n, Nu] = the normal noise of key_alpha, key_critic, key_actor.
+    Every loss sees the parameters from before the update: the critic and the actor use alpha = exp(old log_alpha), the actor the old
+    Q.  The gradient of each loss reaches only its own parameters, so one backward of the sum gives the three gradients."""
+    psizes, qsizes = nets.sac_policy_sizes(O, nu), nets.sac_q_sizes(O, nu)
+    obs, action, reward, discount, next_obs, trunc = unpack_rows(rows, O, nu)
+    x, xn = nets.normalize(obs, mean, std), nets.normalize(next_obs, mean, std)
+    players = nets.unflatten(policy, psizes)
+    logits = nets.relu_mlp(x, players)
+    loc, s = logits.chunk(2, dim=-1)
+    scale = F.softplus(s) + nets.MIN_STD
+    target_entropy = -0.5 * nu
+    raw_a = eps[0] * scale + loc
+    lp_a = nets.log_prob(logits, raw_a)
+    alpha_loss = torch.mean(torch.exp(log_alpha) * (-lp_a - target_entropy).detach())
+    alpha = torch.exp(log_alpha).detach()
+    with torch.no_grad():
+        ln = nets.relu_mlp(xn, nets.unflatten(policy.detach(), psizes))
+        locn, sn = ln.chunk(2, dim=-1)
+        raw_c = eps[1] * (F.softplus(sn) + nets.MIN_STD) + locn
+        next_v = torch.min(nets.sac_q(nets.sac_q_unflatten(target_q, qsizes), xn, torch.tanh(raw_c)), 0).values - alpha * nets.log_prob(ln, raw_c)
+        target = reward * reward_scaling + discount * discounting * next_v
+    qv = nets.sac_q(nets.sac_q_unflatten(q, qsizes), x, action)
+    err = (qv - target) * (1.0 - trunc)
+    critic_loss = 0.5 * torch.mean(err * err)
+    raw_p = eps[2] * scale + loc
+    qa = nets.sac_q(nets.sac_q_unflatten(q.detach(), qsizes), x, torch.tanh(raw_p))
+    actor_loss = torch.mean(alpha * nets.log_prob(logits, raw_p) - torch.min(qa, 0).values)
+    return alpha_loss, critic_loss, actor_loss
+
+
+class Learner:
+    """the parameters (policy, Q, target Q, log_alpha: flat fp32 tensors), their three Adam optimisers (capturable) and Brax's
+    sgd_step: the three losses with the old parameters, the three Adam steps, then target = lerp(target, new Q, tau)"""
+
+    def __init__(self, policy: np.ndarray, q: np.ndarray, O: int, nu: int, learning_rate: float, reward_scaling: float,
+                 discounting: float, tau: float, device):
+        d = torch.device(device)
+        self.O, self.nu, self.reward_scaling, self.discounting, self.tau = O, nu, reward_scaling, discounting, tau
+        self.policy = torch.tensor(np.asarray(policy, np.float32), device=d).requires_grad_(True)    # copies: the caller's arrays stay
+        self.q = torch.tensor(np.asarray(q, np.float32), device=d).requires_grad_(True)
+        self.target_q = self.q.detach().clone()
+        self.log_alpha = torch.zeros(1, device=d, requires_grad=True)
+        cap = d.type == "cuda"
+        for t in (self.policy, self.q, self.log_alpha):
+            t.grad = torch.zeros_like(t)
+        self.opt_alpha = torch.optim.Adam([self.log_alpha], lr=ALPHA_LEARNING_RATE, capturable=cap)
+        self.opt_q = torch.optim.Adam([self.q], lr=learning_rate, capturable=cap)
+        self.opt_policy = torch.optim.Adam([self.policy], lr=learning_rate, capturable=cap)
+
+    def update(self, rows, eps, mean, std):
+        la, lc, lp = losses(self.policy, self.q, self.target_q, self.log_alpha, mean, std, rows, eps, self.O, self.nu,
+                            self.reward_scaling, self.discounting)
+        for t in (self.policy, self.q, self.log_alpha):
+            t.grad.zero_()
+        (la + lc + lp).backward()
+        self.opt_alpha.step()
+        self.opt_q.step()
+        self.opt_policy.step()
+        with torch.no_grad():
+            self.target_q.lerp_(self.q, self.tau)
+
+    def state(self):
+        return [self.policy, self.q, self.target_q, self.log_alpha] + [s for o in (self.opt_alpha, self.opt_q, self.opt_policy)
+                                                                       for st in o.state.values() for s in st.values()]
+
+
+# ---- acting ------------------------------------------------------------------------------------------------------------------------
+class Actor:
+    """The stochastic SAC policy on a VecEnv, with ppo.Actor's protocol: `act(key)` writes tanh(raw) for every env into the VecEnv's
+    actions (one mbd_sac_act launch, make_inference_fn(params)(obs, key) of Brax); start_eval / finish_eval accumulate the return of
+    every env's first episode.  policy: flat fp32 cuda tensor; mean / std: [O] cuda tensors."""
+
+    def __init__(self, venv: VecEnv, policy: torch.Tensor, mean: torch.Tensor, std: torch.Tensor, keys: Optional[torch.Tensor] = None):
+        d = venv.device
+        self.own_key = keys is None
+        self.venv, self.keys = venv, (torch.zeros((1, 2), device=d, dtype=torch.int32) if keys is None else keys)
+        self.ctl = torch.zeros(4, device=d, dtype=torch.int32)
+        self.ret, self.active = torch.zeros(venv.num_envs, device=d), torch.ones(venv.num_envs, device=d)
+        self.policy, self.mean, self.std = policy, mean, std
+        P = _lib.SacPlan()
+        P.B, P.O, P.nu, P.capacity, P.act_key_rows = venv.num_envs, venv.spec.obs_size, venv.spec.nu, venv.num_envs, self.keys.shape[0]
+        P.policy_dev, P.mean_dev, P.std_dev = policy.data_ptr(), mean.data_ptr(), std.data_ptr()
+        P.act_keys_dev, P.act_ctl_dev = self.keys.data_ptr(), self.ctl.data_ptr()
+        P.env_obs_dev, P.env_reward_dev, P.env_done_dev = venv.obs.data_ptr(), venv.reward.data_ptr(), venv.done.data_ptr()
+        P.env_trunc_dev, P.env_actions_dev = venv.truncation.data_ptr(), venv.actions.data_ptr()
+        P.ret_dev, P.active_dev = self.ret.data_ptr(), self.active.data_ptr()
+        self.plan = P
+
+    def start_eval(self):
+        self.ret.zero_()
+        self.active.fill_(1.0)
+        self.ctl.zero_()
+
+    def act(self, key=None):
+        """one acting launch; `key` (uint32 [2]) replaces the table with that single key.  An actor built without a key table must be
+        given a key at every call."""
+        if key is None and self.own_key:
+            raise ValueError("this actor has no key table: pass the key of every act() call")
+        if key is not None:
+            self.keys[0].copy_(_i32(np.asarray(key).reshape(2), self.keys.device))
+            self.ctl.zero_()
+        with torch.cuda.device(self.venv.device):
+            ops.sac_act(self.plan, _lib.SAC_EVAL)
+
+    def finish_eval(self) -> torch.Tensor:
+        with torch.cuda.device(self.venv.device):
+            ops.sac_act(self.plan, _lib.SAC_EVAL_RECORD)
+        return self.ret
+
+
+# ---- the trainer -------------------------------------------------------------------------------------------------------------------
+class SACTrainer:
+    def __init__(self, env, num_timesteps: int, episode_length: int, num_envs: int, num_eval_envs: int, learning_rate: float,
+                 discounting: float, seed: int, batch_size: int, num_evals: int, normalize_observations: bool, reward_scaling: float,
+                 tau: float, min_replay_size: int, max_replay_size: int, grad_updates_per_step: int, device=None):
+        _lib.require_gpu()
+        if not num_envs <= max_replay_size <= _lib.SAC_MAX_CAPACITY:
+            raise ValueError(f"max_replay_size must be in num_envs..{_lib.SAC_MAX_CAPACITY}")
+        self.c = c = counts(num_timesteps, num_envs, min_replay_size, num_evals)
+        self.dev = d = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.env, self.B, self.mb, self.G, self.cap = env, num_envs, batch_size, grad_updates_per_step, max_replay_size
+        self.episode_length, self.normalize_observations = episode_length, normalize_observations
+        self.keys = key_chain(seed, c, num_envs, grad_updates_per_step, num_eval_envs, episode_length)
+        with torch.cuda.device(d):
+            self._setup(num_eval_envs, learning_rate, discounting, reward_scaling, tau)
+
+    def _setup(self, num_eval_envs, learning_rate, discounting, reward_scaling, tau):
+        d, B, G, mb, K = self.dev, self.B, self.G, self.mb, self.keys
+        self.venv = VecEnv(self.env, B, self.episode_length, device=d)
+        self.evenv = VecEnv(self.env, num_eval_envs, self.episode_length, device=d)
+        O, nu = self.venv.spec.obs_size, self.venv.spec.nu
+        if O > _lib.PPO_MAX_OBS or nu > _lib.PPO_MAX_NU:
+            raise ValueError(f"observation size {O} / action size {nu} above {_lib.PPO_MAX_OBS} / {_lib.PPO_MAX_NU}")
+        self.O, self.nu, self.R = O, nu, 2 * O + nu + 3
+        psizes, qsizes = nets.sac_policy_sizes(O, nu), nets.sac_q_sizes(O, nu)
+        self.learner = Learner(nets.init_params(K.policy, psizes), nets.sac_q_init(K.q, qsizes), O, nu, learning_rate, reward_scaling,
+                               discounting, tau, d)
+        f32 = dict(device=d, dtype=torch.float32)
+        self.mean, self.std = torch.zeros(O, **f32), torch.ones(O, **f32)
+        self.stat = torch.zeros(1 + 2 * O, device=d, dtype=torch.float64)
+        self.stat_scratch = torch.zeros(((B + _lib.PPO_STAT_ROWS - 1) // _lib.PPO_STAT_ROWS) * 2 * O, device=d, dtype=torch.float64)
+        self.stage = torch.zeros((B, O), **f32)
+        self.ring = torch.zeros((self.cap, self.R), **f32)
+        self.ring_ctl = torch.zeros(4, device=d, dtype=torch.int32)
+        self.sample_ctl = torch.zeros(4, device=d, dtype=torch.int32)
+        self.sample_ctl[2:4].copy_(_i32(K.buffer, d))
+        self.act_keys = _i32(K.act, d)
+        self.act_ctl = torch.zeros(4, device=d, dtype=torch.int32)
+        self.noise_keys = _i32(K.noise.reshape(-1), d)
+        self.idx = torch.zeros(G * mb, device=d, dtype=torch.int32)
+        self.batch = torch.zeros((G, mb, self.R), **f32)
+        self.eps = torch.zeros((3, G, mb, nu), **f32)
+        self.upd_ctl = torch.zeros(1, device=d, dtype=torch.int64)
+        v = self.venv
+        P = _lib.SacPlan()
+        P.B, P.O, P.nu, P.capacity, P.batch, P.updates = B, O, nu, self.cap, mb, G
+        P.act_key_rows, P.noise_key_rows = self.act_keys.shape[0], K.noise.shape[0]
+        P.policy_dev, P.mean_dev, P.std_dev = self.learner.policy.data_ptr(), self.mean.data_ptr(), self.std.data_ptr()
+        P.act_keys_dev, P.act_ctl_dev = self.act_keys.data_ptr(), self.act_ctl.data_ptr()
+        P.env_obs_dev, P.env_reward_dev, P.env_done_dev = v.obs.data_ptr(), v.reward.data_ptr(), v.done.data_ptr()
+        P.env_trunc_dev, P.env_actions_dev = v.truncation.data_ptr(), v.actions.data_ptr()
+        P.stage_obs_dev, P.ring_dev, P.ring_ctl_dev, P.sample_ctl_dev = (t.data_ptr() for t in (self.stage, self.ring, self.ring_ctl,
+                                                                                                  self.sample_ctl))
+        P.noise_keys_dev, P.idx_dev, P.batch_dev, P.eps_dev = (t.data_ptr() for t in (self.noise_keys, self.idx, self.batch, self.eps))
+        self.plan = P
+        S = _lib.PpoPlan()         # running_statistics.update over the B acting observations: PPO's launch with one slot
+        S.B, S.O, S.nu, S.slots = B, O, nu, 1
+        S.obs_dev, S.stat_dev, S.stat_scratch_dev = self.stage.data_ptr(), self.stat.data_ptr(), self.stat_scratch.data_ptr()
+        S.mean_dev, S.std_dev = self.mean.data_ptr(), self.std.data_ptr()
+        self.stat_plan = S
+        self.eval_keys = _i32(K.eval_act.reshape(-1, 2), d)
+        self.eval_reset = _i32(K.eval_reset, d)
+        self.actor = Actor(self.evenv, self.learner.policy.detach(), self.mean, self.std, self.eval_keys)
+        self.venv.reset(_i32(K.env, d))
+        self.step_index = 0
+        self.eval_index = 0
+        self._act_graph = self._sample_graph = self._sgd_graph = self._eval_graph = None
+
+    # -- the pieces ------------------------------------------------------------------------------------------------------------------
+    def actor_step(self):
+        """acting.actor_step + running_statistics.update + insert: act, env step, record, statistics"""
+        ops.sac_act(self.plan, _lib.SAC_ACT)
+        ops.vec_step(self.venv.plan)
+        ops.sac_record(self.plan)
+        if self.normalize_observations:
+            ops.ppo_obs_stats(self.stat_plan)
+
+    def sample(self):
+        ops.sac_sample(self.plan)
+        self.upd_ctl.zero_()
+
+    def sgd_step(self):
+        """update upd_ctl of the training step: its batch and noise, Brax's sgd_step, then upd_ctl += 1"""
+        with torch.no_grad():
+            rows = torch.index_select(self.batch.view(self.G, -1), 0, self.upd_ctl).view(self.mb, self.R)
+            eps = torch.index_select(self.eps.view(3, self.G, -1), 1, self.upd_ctl).view(3, self.mb, self.nu)
+        self.learner.update(rows, eps, self.mean, self.std)
+        with torch.no_grad():
+            self.upd_ctl.add_(1)
+
+    def prefill(self):
+        """prefill_replay_buffer: num_prefill_actor_steps acting steps with the initial policy"""
+        with torch.cuda.device(self.dev):
+            for _ in range(self.c.prefill_steps):
+                self._act_graph.replay() if self._act_graph is not None else self.actor_step()
+
+    def capture(self):
+        """captures the acting step, the sampling and one update as CUDA graphs (and the evaluation step).  The update is warmed up
+        on a side stream first and every state it touched is restored, so capturing changes no result."""
+        with torch.cuda.device(self.dev):
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self.actor_step()
+            self._act_graph = g
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self.sample()
+            self._sample_graph = g
+            L = self.learner
+            kept = (L.policy, L.q, L.target_q, L.log_alpha, self.upd_ctl)
+            snap = [t.detach().clone() for t in kept]
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                for _ in range(2):
+                    self.sgd_step()
+            torch.cuda.current_stream().wait_stream(s)
+            with torch.no_grad():
+                for t, v in zip(kept, snap):
+                    t.copy_(v)
+                for t in L.state()[4:]:     # the optimisers' moments and step counts
+                    t.zero_()
+                for t in (L.policy.grad, L.q.grad, L.log_alpha.grad):
+                    t.zero_()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self.sgd_step()
+            self._sgd_graph = g
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self.actor.act()
+                ops.vec_step(self.evenv.plan)
+            self._eval_graph = g
+
+    def training_step(self):
+        """Brax's training_step: an actor step, the replay sample, grad_updates_per_step updates"""
+        if self.step_index >= self.keys.noise.shape[0]:
+            raise RuntimeError("every training step of the key chain has run")
+        with torch.cuda.device(self.dev):
+            self._act_graph.replay() if self._act_graph is not None else self.actor_step()
+            self._sample_graph.replay() if self._sample_graph is not None else self.sample()
+            for _ in range(self.G):
+                self._sgd_graph.replay() if self._sgd_graph is not None else self.sgd_step()
+        self.step_index += 1
+
+    def env_steps(self) -> int:
+        return self.c.prefill_env_steps + self.step_index * self.B
+
+    def evaluate(self) -> float:
+        """Evaluator.run_evaluation (PPO's): num_eval_envs envs, episode_length stochastic steps, the mean return of every env's
+        first episode (synchronises)"""
+        with torch.cuda.device(self.dev):
+            self.evenv.reset(self.eval_reset[self.eval_index])
+            self.actor.start_eval()
+            self.actor.ctl[1:2].fill_(self.eval_index * self.episode_length)
+            for _ in range(self.episode_length):
+                if self._eval_graph is not None:
+                    self._eval_graph.replay()
+                else:
+                    self.actor.act()
+                    ops.vec_step(self.evenv.plan)
+            ret = self.actor.finish_eval()
+            out = float(ret.mean().item())
+        self.eval_index += 1
+        return out
+
+    def params(self) -> dict:
+        L = self.learner
+        return dict(policy=L.policy.detach().cpu().numpy(), q=L.q.detach().cpu().numpy(), target_q=L.target_q.cpu().numpy(),
+                    log_alpha=L.log_alpha.detach().cpu().numpy(), mean=self.mean.cpu().numpy(), std=self.std.cpu().numpy(),
+                    stat=self.stat.cpu().numpy())
+
+
+def train(environment, num_timesteps: int, episode_length: int, action_repeat: int = 1, num_envs: int = 1, num_eval_envs: int = 128,
+          learning_rate: float = 1e-4, discounting: float = 0.9, seed: int = 0, batch_size: int = 256, num_evals: int = 1,
+          normalize_observations: bool = False, max_devices_per_host: Optional[int] = None, reward_scaling: float = 1.0,
+          tau: float = 0.005, min_replay_size: int = 0, max_replay_size: Optional[int] = None, grad_updates_per_step: int = 1,
+          deterministic_eval: bool = False, progress_fn: Callable[[int, dict], None] = lambda *a: None, capture: bool = True):
+    """sac.train with Brax's signature and defaults for the arguments the reference passes.  Returns (make_inference_fn, params,
+    metrics): make_inference_fn(params) gives an `Actor` factory for a VecEnv; params is a dict of numpy arrays (policy, q, target_q,
+    log_alpha, the observation statistics).  One device: max_devices_per_host is accepted and has nothing to choose."""
+    if action_repeat != 1:
+        raise NotImplementedError("action_repeat != 1 is not built (the vector env steps once per action)")
+    if deterministic_eval:
+        raise NotImplementedError("only the stochastic evaluation of the reference's config is built")
+    if max_replay_size is None:
+        max_replay_size = num_timesteps
+    env = get_env(environment) if isinstance(environment, str) else environment
+    tr = SACTrainer(env, num_timesteps, episode_length, num_envs, num_eval_envs, learning_rate, discounting, seed, batch_size, num_evals,
+                    normalize_observations, reward_scaling, tau, min_replay_size, max_replay_size, grad_updates_per_step)
+    if capture:
+        tr.capture()
+    c = tr.c
+    metrics = {}
+    if num_evals > 1:
+        metrics = {"eval/episode_reward": tr.evaluate()}
+        progress_fn(0, metrics)
+    tr.prefill()
+    for _ in range(c.num_evals_after_init):
+        t0 = time.perf_counter()
+        for _ in range(c.steps_per_epoch):
+            tr.training_step()
+        torch.cuda.synchronize(tr.dev)
+        sps = c.steps_per_epoch * c.env_steps_per_training_step / (time.perf_counter() - t0)
+        metrics = {"eval/episode_reward": tr.evaluate(), "training/sps": sps}
+        progress_fn(tr.env_steps(), metrics)
+    params = tr.params()
+
+    def make_inference_fn(p):
+        def make(venv: VecEnv) -> Actor:
+            d = venv.device
+            return Actor(venv, torch.from_numpy(p["policy"]).to(d), torch.from_numpy(p["mean"]).to(d), torch.from_numpy(p["std"]).to(d))
+        return make
+
+    return make_inference_fn, params, metrics

@@ -3,14 +3,14 @@
 Trains PPO (mbd_b200.rl.ppo) with the reference's per-env hyperparameters, prints `step: N, episode return: X` at every evaluation,
 `time to jit`, `time to train`, saves the parameters to results/{env}/params.npz (Brax's pickle format is not reproduced), runs the
 reference's final evaluation (8 episodes of 50 steps, 40 for pushT, one env, the reference's key chain) and writes results/{env}/RL.html.
-Extensions: --num_timesteps and --seed override the table for short runs.  hopper (SAC in the reference) is not built; pusher fails
-in get_env as in the reference.  ant trains without Brax's unhealthy termination: the host Ant and the vector env never terminate.
+Extensions: --num_timesteps and --seed override the table for short runs.  hopper, which the reference trains with SAC, has its own
+script (python -m mbd_b200.rl.train_sac --env_name hopper); pusher fails in get_env as in the reference.  ant trains without Brax's
+unhealthy termination: the host Ant and the vector env never terminate.
 """
 from __future__ import annotations
 
 import argparse
 import os
-from datetime import datetime
 
 import numpy as np
 
@@ -43,15 +43,9 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=None, help="override the table's seed")
     a = ap.parse_args(argv)
     if a.env_name in SAC_ENVS:
-        raise SystemExit(f"{a.env_name}: the reference trains it with Brax SAC, which is not built here (only PPO is)")
+        raise SystemExit(f"{a.env_name}: the reference trains it with Brax SAC, not PPO: run python -m mbd_b200.rl.train_sac --env_name {a.env_name}")
 
-    import torch
-
-    import mbd_b200
-    from .. import prng
     from ..envs import get_env
-    from ..envs.vec import VecEnv
-    from ..io import brax_json
     from . import ppo
 
     env = get_env(a.env_name)       # pusher raises here, as in the reference
@@ -62,29 +56,45 @@ def main(argv=None):
         cfg["num_timesteps"] = a.num_timesteps
     if a.seed is not None:
         cfg["seed"] = a.seed
-    rng = prng.PRNGKey(0)
-    rng, rng_reset = prng.split2(rng)
+    progress, times = progress_printer()
+    make_inference_fn, params, _ = ppo.train(environment=env, progress_fn=progress, **cfg)
+    post_training(a.env_name, env, make_inference_fn, params, times)
 
-    xdata, ydata = [], []
+
+def progress_printer():
+    """the reference's progress_fn: prints `step: N, episode return: X` and records the time of every evaluation"""
+    from datetime import datetime
     times = [datetime.now()]
 
     def progress(num_steps, metrics):
         times.append(datetime.now())
-        xdata.append(num_steps)
-        ydata.append(metrics["eval/episode_reward"])
         print(f"step: {num_steps}, episode return: {metrics['eval/episode_reward']:.2f}", flush=True)
 
-    make_inference_fn, params, _ = ppo.train(environment=env, progress_fn=progress, **cfg)
+    return progress, times
+
+
+def post_training(env_name, env, make_inference_fn, params, times):
+    """the reference script's tail after training: the times, results/{env}/params.npz, the mean reward of 8 episodes of 50 steps
+    (40 for pushT) on one env with the reference's key chain, and results/{env}/RL.html of one more rollout"""
+    import torch
+
+    import mbd_b200
+    from .. import prng
+    from ..envs.vec import VecEnv
+    from ..io import brax_json
+
+    rng = prng.PRNGKey(0)
+    rng, rng_reset = prng.split2(rng)
     print(f"time to jit: {times[1] - times[0]}")
     print(f"time to train: {times[-1] - times[1]}")
 
-    path = f"{mbd_b200.__path__[0]}/../results/{a.env_name}"
+    path = f"{mbd_b200.__path__[0]}/../results/{env_name}"
     os.makedirs(path, exist_ok=True)
     np.savez(f"{path}/params.npz", **params)
 
     venv = VecEnv(env, 1)
     actor = make_inference_fn(params)(venv)
-    nstep = 40 if a.env_name == "pushT" else 50
+    nstep = 40 if env_name == "pushT" else 50
     rew = []
     for _ in range(8):
         rng, rng_i = prng.split2(rng)
