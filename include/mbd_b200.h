@@ -21,7 +21,6 @@ extern "C" {
 #define MBD_EINVAL (-1)  /* bad argument / bad blob */
 #define MBD_ECUDA (-2)   /* CUDA runtime error (see mbd_last_error) */
 #define MBD_ENOGPU (-3)  /* no CUDA device: there is deliberately NO CPU fallback */
-#define MBD_EUNSUPPORTED (-4) /* this fused entry point does not cover the configuration: use the separate calls */
 
 typedef struct mbd_model mbd_model;
 typedef void* mbd_stream; /* cudaStream_t */
@@ -32,13 +31,11 @@ int mbd_layout_info(int32_t* out, int n);
 int mbd_abi_sizes(int32_t* out, int n);
 const char* mbd_last_error(void);
 int mbd_device_count(void);
-/* rollout kernel mapping: 0 = auto (by shard size), 1 = v1 (one link per lane), 2/3 = v2 (one link per
- * warp, lane = sample) with CTA-wide / named-barrier phase synchronisation (4, mbarrier polling, was removed), 5 = v2 with two
- * same-type links per warp (16 samples per CTA), 6 = v2 with two interleaved 32-sample groups per 704-thread CTA
- * (leaf links decoupled from the group barriers), 8/9 = packed kernel: two samples per lane (two independent chains per thread),
- * 64 samples per CTA, group barriers / named edge barriers (11-link models; others fall back to 2).  4 and 7 are unused
- * (as are 10 / 11, a round-2 experiment that lost and was removed).
- * All variants produce bit-identical results; the switch exists for tests and profiling. */
+/* rollout kernel mapping: 0 = auto (by shard size), 1 = v1 (one link per lane), 2 / 3 = v2 (one link per warp, lane = sample)
+ * with CTA-wide / named-barrier phase synchronisation, 8 = packed kernel: two samples per lane (two independent chains per
+ * thread), 64 samples per CTA, group barriers with decoupled leaves.  Fallbacks: 3 runs 2 on a tree that needs more than 15
+ * named barriers; 8 runs 2 on a model that is not 11 hinge-only links with at most 2 contacts per link.  Any other value is
+ * MBD_EINVAL.  All variants produce bit-identical results; the switch exists for tests and profiling. */
 int mbd_set_kernel_variant(int v);
 /* threefry counter layout of every in-kernel sampler (process-wide): 0 = legacy (jax_threefry_partitionable=False, what the JAX
  * known-answer vectors in tests/test_prng.py pin), 1 = partitionable (the default of JAX >= 0.5; [jax-recalled], unpinned).
@@ -46,10 +43,6 @@ int mbd_set_kernel_variant(int v);
 int mbd_set_prng_layout(int partitionable);
 /* tuning hook: slot -> link order of the one-link-per-warp mapping (slot L-1 gets the highest warp id) */
 int mbd_model_set_warp_order(mbd_model* m, const int* order, int n);
-/* tuning hook: cycles the second sample group of a two-group CTA waits before its first step (de-phases the groups) */
-int mbd_set_group_stagger(int cycles);
-/* tuning hook: two-group CTA warp table, map[w] = (group << 4) | slot for the 2*L warps */
-int mbd_model_set_group_map(mbd_model* m, const int* map, int n);
 
 /* brax.io.mjcf.load(...) result made device resident — replaces the `sys` captured by the
  * jitted env.step (upstream mbd/envs/humanoidrun.py:15-17).  blob: include/mbd_model.h */
@@ -77,16 +70,6 @@ int mbd_rollout(const mbd_model* m, const float* state_init_dev, const float* Y0
 int mbd_sample_rollout(const mbd_model* m, const float* state_init_dev, const uint32_t key[2], int n_total,
                        int n_begin, int n_local, int H, float sigma, const float* Ybar_dev, float* Y0s_dev,
                        float* rews_dev, const float* xref_dev, int href, float* logpd_dev, mbd_stream s);
-
-/* The whole of reverse_once (mbd_planner.py:97-135, enable_demo False, one GPU) as ONE cooperative kernel:
- * sampling + rollouts, grid barrier, reward statistics + softmax (recomputed per CTA), weighted-mean runs, grid
- * barrier, pairwise tree + update.  Bit-identical to mbd_sample_rollout + mbd_softmax_weights + mbd_weighted_sum
- * + mbd_update.  Returns MBD_EUNSUPPORTED when the configuration is not covered (model shape, shard too large
- * for co-residency or too small to benefit): the caller then uses the separate entry points.
- * runs_dev: ceil(n/64)*H*Nu floats; scalars_dev[4] as in mbd_softmax_weights. */
-int mbd_reverse_step(const mbd_model* m, const float* state_init_dev, const uint32_t key[2], int n, int H, float sigma,
-                     const float* Ybar_i_dev, float temp, const float coef[5], float* Y0s_dev, float* rews_dev,
-                     float* weights_dev, float* scalars_dev, float* runs_dev, float* Ybar_im1_dev, mbd_stream s);
 
 /* Car2d (self-contained env, upstream mbd/envs/car2d.py:77-102).
  * params_dev: [obs_center(11x2), obs_radius, dt, dt/2, dt/6]; x0_dev [3]; xref_dev [href,2] or NULL.
@@ -120,15 +103,6 @@ int mbd_weighted_sum_runs(const float* weights_dev, const float* Y0s_dev, int n_
  * upstream mbd/planners/path_integral.py:39-45, same deterministic order as mbd_weighted_sum. */
 int mbd_weighted_sqerr_sum(const float* weights_dev, const float* Y0s_dev, const float* mu_dev, int n_local, int HNu,
                            float* scratch_dev, float* partial_dev, mbd_stream s);
-
-/* Fused exchange over NVLink peer memory (replaces ncclAllGather for the two small per-step exchanges of
- * reverse_once when the Nsample axis is sharded): an in-kernel cross-GPU barrier (system-scope flags in
- * the peers' symmetric buffers) followed by direct peer loads.  peer_base_ptrs [P] are the base addresses
- * of every rank's symmetric buffer (identical layout); dst_dev [P*count] receives rank-ordered data read
- * from word offset src_off_words; flag rows live at flag_off_words (P words, zero-initialised, one row
- * per call site); epoch must increase by one per call on the same row.  err_dev: set to 1 on timeout. */
-int mbd_peer_gather(const uint64_t* peer_base_ptrs, int P, int rank, size_t src_off_words, int count,
-                    size_t flag_off_words, uint32_t epoch, float* dst_dev, uint32_t* err_dev, mbd_stream s);
 
 /* Test hook: element-wise MBD_DIV (op 0), MBD_RCP (1), MBD_SQRT (2), mbd_atan2f (3) — the branch-free
  * exact device sequences of include/mbd_fp32.h — so tests can compare them with IEEE results bit for bit; and the

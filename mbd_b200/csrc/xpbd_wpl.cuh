@@ -38,13 +38,9 @@ constexpr int kEF = 7;   // exchange fields per link: T(3)  |  dpp(3) dqp(4)
 struct WplSmem {
   float* X;  // [L][kXF][32]
   float* E;  // [L][kEF][32]
-  int lane;  // sample slot inside a row, WITHOUT the half-warp offset of the row's owner
-  // Row of link k holds its samples at [off(k) + lane]; off(k) = 0 when a warp owns one link (SPLIT 1) or
-  // 16 * (half of the warp that owns k) when two links share a warp (SPLIT 2).  Packed 4 bits per link.
-  unsigned long long offs;
-  __device__ __forceinline__ int off(int link) const { return (int)((offs >> (4 * link)) & 0xFull) << 2; }
-  __device__ __forceinline__ float& x(int link, int f) const { return X[(link * kXF + f) * kWplLanes + off(link) + lane]; }
-  __device__ __forceinline__ float& e(int link, int f) const { return E[(link * kEF + f) * kWplLanes + off(link) + lane]; }
+  int lane;  // sample slot inside a row
+  __device__ __forceinline__ float& x(int link, int f) const { return X[(link * kXF + f) * kWplLanes + lane]; }
+  __device__ __forceinline__ float& e(int link, int f) const { return E[(link * kEF + f) * kWplLanes + lane]; }
   __device__ __forceinline__ v3 xp(int link) const { return V3(x(link, 0), x(link, 1), x(link, 2)); }
   __device__ __forceinline__ q4 xq(int link) const { return Q4(x(link, 3), x(link, 4), x(link, 5), x(link, 6)); }
   __device__ __forceinline__ v3 xw(int link) const { return V3(x(link, 7), x(link, 8), x(link, 9)); }
@@ -65,16 +61,6 @@ struct WarpCfg {
   int l, ndof, parent, ncon, smask;   // smask: bit k = dof k is a slide dof (world-parented links only)
   int child[MBD_MAXCHILD];
 };
-
-__device__ __forceinline__ void load_warp_cfg(const ModelSmem& M, int l, WarpCfg& c) {
-  c.l = l;
-  c.ndof = M.li(MBD_F_NDOF, l);
-  c.parent = M.li(MBD_F_PARENT, l);
-  c.ncon = M.li(MBD_F_NCON, l);
-  c.smask = c.ndof > 0 ? M.li(MBD_F_SLIDE, l) : 0;
-#pragma unroll
-  for (int k = 0; k < MBD_MAXCHILD; ++k) c.child[k] = M.li(MBD_F_CHILD0 + k, l);
-}
 
 // axis_angle_ang specialised for 1-dof links: only psi and the extra matrix entries are used
 // (oracle computes the rest and discards it — same bits for what is used).
@@ -104,21 +90,20 @@ struct SyncCta {
   template <class C> __device__ __forceinline__ void end_D(const C&) { phase_end(); }
 };
 
-// SyncGroup: a CTA that hosts G independent sample groups gives each group its own hardware barrier ids;
-// within a group the phases are separated by group-wide barriers, except that LEAF links never hold anybody up
-// where nobody depends on them:
+// SyncGroup: the packed kernel's sync.  The phases are separated by CTA-wide named barriers (ids base .. base+3),
+// except that LEAF links never hold anybody up where nobody depends on them:
 //   * after A and after C a leaf only bar.arrive's (the next phase, B or D, gathers from CHILDREN: a leaf has none,
 //     so it runs straight on; its parent still sees the leaf's terms because the arrival publishes them);
 //   * after D the leaves with contacts ("late" leaves: their D phase is several times longer than anybody else's)
-//     are left out of the group barrier: everybody else syncs on id_x and then bar.arrive's on id_y, the late
+//     are left out of the barrier: everybody else syncs on id_x and then bar.arrive's on id_y, the late
 //     leaves bar.sync on id_y — they wait for their parent's pose, nobody waits for them until the end of the
 //     next A phase, which therefore overlaps the contact solve.
 // Hazards: a leaf's X row is read by nobody; its E row is read by the parent in B and D, and rewritten by the leaf
-// only in C (after the group-wide B->C barrier) and in A (after id_y, i.e. after the parent finished D).
+// only in C (after the CTA-wide B->C barrier) and in A (after id_y, i.e. after the parent finished D).
 template <int NL>
 struct SyncGroup {
   // ids base+0: after A and after C; base+1: after B; base+2 / base+3: after D.  A warp never touches the same id
-  // twice without a blocking group-wide barrier on ANOTHER id in between (a hardware barrier has one arrival
+  // twice without a blocking CTA-wide barrier on ANOTHER id in between (a hardware barrier has one arrival
   // counter: a second arrival of the same warp would be counted into the generation that is still open).
   // bar.arrive orders the warp's earlier shared-memory writes before the barrier completes (CUTLASS NamedBarrier idiom).
   int base, count_x;   // count_x = 32 * (links that are not late leaves)
@@ -147,21 +132,13 @@ struct SyncGroup {
 //   pose id : the node bar.arrive's, each child bar.sync's      (count = 32 * (1 + nchildren))
 //   terms id: each child bar.arrive's, the node bar.sync's      (same count)
 // Needs 2 * (#nodes with children) <= 15; otherwise the caller falls back to SyncCta.
-template <bool FENCE>
-struct SyncNamedT {
+struct SyncNamed {
   int my_pose_id, my_terms_id, my_count;       // valid when this link has children (else 0)
   int par_pose_id, par_terms_id, par_count;    // ids owned by the parent (0 when parent is the world / none)
   // No fence before the arrival: bar.arrive / bar.sync order the arriving thread's earlier shared-memory accesses before the
   // barrier completes for every participant (the PTX ISA's own producer / consumer example is st.shared; bar.arrive on one side,
   // bar.sync; ld.shared on the other).  Round 1 had a __threadfence_block() here = four MEMBAR.SC.CTA per warp and substep.
-  // FENCE: kept in the packed kernel, dropped in the scalar one; both are correct either way, and scripts/gpu_fence_ab.py times
-  // the two builds alternately on one GPU.
   static __device__ __forceinline__ void bar_arrive(int id, int count) {
-#ifdef MBD_NAMED_FENCE   // the A/B switch: force the fence everywhere
-    __threadfence_block();
-#else
-    if (FENCE) __threadfence_block();
-#endif
     asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
   }
   static __device__ __forceinline__ void bar_sync(int id, int count) {
@@ -208,8 +185,6 @@ struct SyncNamedT {
     return 2 * nparents <= 15;
   }
 };
-using SyncNamed = SyncNamedT<false>;        // scalar warp-per-link kernels
-using SyncNamedFenced = SyncNamedT<true>;   // packed kernel
 
 // One brax.positional.pipeline.step for (link = this warp, sample = this lane).
 // All threads of the CTA must call.

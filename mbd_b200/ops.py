@@ -35,9 +35,8 @@ def _dev(t: torch.Tensor, dtype=torch.float32) -> torch.Tensor:
 
 
 def set_kernel_variant(v: int):
-    """0 = auto, 1 = lane-per-link kernel, 2/3/4 = warp-per-link kernel with CTA / named / mbarrier sync,
-    5 = two links per warp / 16 samples per CTA,
-    6 = two interleaved sample groups per CTA (all bit-identical)."""
+    """0 = auto, 1 = lane-per-link kernel, 2/3 = warp-per-link kernel with CTA / named-barrier sync,
+    8 = packed kernel, two samples per lane (all bit-identical; 3 and 8 fall back to 2 on models they do not cover)."""
     check(_lib.lib().mbd_set_kernel_variant(int(v)), "mbd_set_kernel_variant")
 
 
@@ -111,24 +110,6 @@ def sample_rollout(model: Model, state_init, key, n_total, n_begin, n_local, H, 
                                         _stream()), "mbd_sample_rollout")
 
 
-EUNSUPPORTED = -4
-
-
-def reverse_step(model: Model, state_init, key, n, H, sigma, Ybar_i, temp, coef, Y0s_out, rews_out, weights_out, scalars_out,
-                 runs_scratch, out) -> bool:
-    """reverse_once as ONE cooperative kernel.  Returns False when the configuration is not covered by the
-    fused kernel (the caller then issues the separate launches)."""
-    k, kp = key_ptr(key)
-    c = (ctypes.c_float * 5)(*[float(v) for v in coef])
-    rc = _lib.lib().mbd_reverse_step(model.handle, _p(_dev(state_init)), kp, n, H, ctypes.c_float(sigma), _p(_dev(Ybar_i)),
-                                     ctypes.c_float(temp), c, _p(_dev(Y0s_out)), _p(_dev(rews_out)), _p(_dev(weights_out)),
-                                     _p(_dev(scalars_out)), _p(_dev(runs_scratch)), _p(_dev(out)), _stream())
-    if rc == EUNSUPPORTED:
-        return False
-    check(rc, "mbd_reverse_step")
-    return True
-
-
 def car2d_rollout(params, x0, Y0s, xref=None, want_rewss=False, want_traj=False, key=None, n_total=0, n_begin=0,
                   sigma=0.0, Ybar=None, rews_out=None, logpd_out=None):
     """Car2d rollouts; with `key` the noise is drawn in-kernel and written to Y0s [n,H,2]."""
@@ -193,12 +174,6 @@ def weighted_sqerr_sum(weights, Y0s, mu, HNu, scratch, partial_out):
     n_local = weights.numel()
     check(_lib.lib().mbd_weighted_sqerr_sum(_p(_dev(weights)), _p(_dev(Y0s)), _p(_dev(mu)), n_local, HNu, _p(_dev(scratch)),
                                             _p(_dev(partial_out)), _stream()), "mbd_weighted_sqerr_sum")
-
-
-def peer_gather(peer_ptrs, P, rank, src_off_words, count, flag_off_words, epoch, dst, err):
-    arr = (ctypes.c_uint64 * P)(*[int(p) for p in peer_ptrs])
-    check(_lib.lib().mbd_peer_gather(arr, P, rank, src_off_words, count, flag_off_words, ctypes.c_uint32(epoch), _p(_dev(dst)),
-                                     ctypes.c_void_p(err.data_ptr()), _stream()), "mbd_peer_gather")
 
 
 def update(partials, P, HNu, Ybar_i, coef, out):

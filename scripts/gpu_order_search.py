@@ -1,11 +1,11 @@
-"""Random search over the warp -> link order of the packed kernel (variant 9): which links share an SM sub-partition scheduler
+"""Random search over the warp -> link order of the packed kernel (variant 8): which links share an SM sub-partition scheduler
 (warp id % 4) and which get the high warp ids the arbiter favours.  Every order is bit-identical; only the time changes."""
 import ctypes, json, os, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import mbd_b200
 from mbd_b200 import ops, prng, _lib
-variant = int(sys.argv[1]) if len(sys.argv) > 1 else 9
+variant = int(sys.argv[1]) if len(sys.argv) > 1 else 8
 trials = int(sys.argv[2]) if len(sys.argv) > 2 else 60
 env = mbd_b200.envs.get_env("humanoidrun")
 st = torch.as_tensor(env.reset(prng.split(prng.PRNGKey(0))[1]).pipeline_state.raw, device="cuda:0")

@@ -19,7 +19,7 @@ L = _lib.lib()
 key = np.uint32([1, 2])
 names = env.sys.link_names
 for n in (int(os.environ.get("MBD_PROF_N", "8192")),):
-    for v in ([int(x) for x in sys.argv[1:]] or [2, 6]):
+    for v in ([int(x) for x in sys.argv[1:]] or [2, 8]):
         ops.set_kernel_variant(v)
         Y0s = torch.empty((n, 850), device="cuda:0"); rews = torch.empty(n, device="cuda:0"); Yb = torch.zeros(850, device="cuda:0")
         ops.sample_rollout(m, st, key, n, 0, n, 50, 0.88, Yb, Y0s, rews); torch.cuda.synchronize()

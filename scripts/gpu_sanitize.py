@@ -18,7 +18,7 @@ n, H = 64, 5
 us = torch.as_tensor(np.clip(np.random.default_rng(0).normal(size=(n, H, 17)), -1, 1).astype(np.float32), device="cuda:0")
 if which in ("all", "rollout"):
     ref = None
-    for v in (2, 1, 3, 5, 6, 8, 9):
+    for v in (2, 1, 3, 8):
         ops.set_kernel_variant(v)
         out = ops.rollout(m, sti, us, want_final=True)["final"].cpu().numpy()
         ref = out if ref is None else ref

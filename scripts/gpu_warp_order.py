@@ -25,7 +25,7 @@ for name, order in ORDERS.items():
     if order is not None:
         arr = (ctypes.c_int * 11)(*order)
         _lib.check(_lib.lib().mbd_model_set_warp_order(m.handle, arr, 11), "set order")
-    for v in (6, 2):
+    for v in (8, 2):
         ops.set_kernel_variant(v)
         for _ in range(2): ops.sample_rollout(m, st, key, n, 0, n, 50, 0.88, Yb, Y0s, rews)
         torch.cuda.synchronize()

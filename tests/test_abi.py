@@ -29,6 +29,18 @@ def test_exports_every_declared_symbol():
     assert sorted(_lib.EXPORTS) == names
 
 
+def test_kernel_variant_accepts_only_the_kept_kernels():
+    """mbd_set_kernel_variant takes auto (0) and the variants 1, 2, 3 and 8; every other value is MBD_EINVAL"""
+    L = _lib.lib()
+    try:
+        for v in (0, 1, 2, 3, 8):
+            assert L.mbd_set_kernel_variant(v) == 0, v
+        for v in (4, 5, 6, 7, 9, 10):
+            assert L.mbd_set_kernel_variant(v) == -1, v
+    finally:
+        L.mbd_set_kernel_variant(0)
+
+
 def test_layout_matches_python_packer():
     out = np.zeros(64, np.int32)
     n = _lib.lib().mbd_layout_info(out.ctypes.data_as(_lib.c_i32p), 64)

@@ -109,7 +109,7 @@ def test_env_kind_matches_solo(env_name, B, Ns, H, Nd, demo):
 
 
 # ---- 2. every explicit kernel variant --------------------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", [1, 2, 3, 5, 6, 8, 9])
+@pytest.mark.parametrize("variant", [1, 2, 3, 8])
 def test_kernel_variants_ragged(variant):
     """B = 3 at a ragged N = 100 on humanoidrun: every variant's batched launch equals the stand-alone solves"""
     env = mbd_b200.envs.get_env("humanoidrun")

@@ -86,7 +86,7 @@ def _check_all_variants(orc, env, facts, seed, n=77, H=6):
     m = env.device_model(dev)
     st_d = torch.as_tensor(raw, device=dev)
     Y_d = torch.as_tensor(Y, device=dev)
-    for v in (0, 1, 2, 3, 5, 6, 8, 9):
+    for v in (0, 1, 2, 3, 8):
         ops.set_kernel_variant(v)
         try:
             out = ops.rollout(m, st_d, Y_d, want_rewss=True, want_final=True)
@@ -112,7 +112,7 @@ def test_rollout_kernels_on_the_topologies_the_barrier_protocols_special_case(or
 @pytest.mark.gpu
 @pytest.mark.parametrize("seed", SEEDS + SEEDS11)
 def test_rollout_kernels_match_oracle_on_random_models(orc, tmp_path, seed):
-    """every kernel mapping (auto, lane-per-link, warp-per-link with CTA / named / group barriers, split warps, packed two-sample;
+    """every kernel mapping (auto, lane-per-link, warp-per-link with CTA / named barriers, packed two-sample with group barriers;
     variants that do not apply to a model fall back inside the library) == oracle, bit for bit, on a ragged sample count
     (77: two full 32-sample groups and a partial one; one full and one partial 64-sample packed CTA)"""
     env, facts = _env(tmp_path, seed, links=11 if seed >= 100 else 0)

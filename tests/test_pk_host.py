@@ -140,4 +140,4 @@ def test_no_packed_contraction_in_the_product_kernels():
         pytest.skip("CUDA toolkit not available")
     r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "check_pk_contraction.py")], capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
-    assert r.stdout.count(" ok") >= 8
+    assert r.stdout.count(" ok") >= 3   # fused, non-fused and batched instantiations

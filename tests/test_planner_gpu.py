@@ -126,7 +126,7 @@ def test_shard_count_invariance_bit_exact(humanoidrun_setup, P, demo):
 
 def test_exchange_timeout_poisons_the_output(humanoidrun_setup, monkeypatch):
     """a peer that never shows up: the rendezvous times out, ctl.err is set and the step's outputs are NaN — a stale
-    or missing exchange can never be mistaken for a result (ADVICE r1: k_peer_gather used stale data after a timeout)"""
+    or missing exchange can never be mistaken for a result (ADVICE r1: the former peer-gather kernel used stale data after a timeout)"""
     monkeypatch.setenv("MBD_XCHG_TIMEOUT_S", "0.005")
     env, blob, st = humanoidrun_setup
     _, alphas, alphas_bar, sigmas = opl.make_schedule(1e-4, 1e-2, 10)
@@ -256,34 +256,3 @@ def test_run_path_integral_cli_surface(capsys):
     assert mus.shape == (5, 50, 2) and np.isfinite(rf) and "override temp_sample" in capsys.readouterr().out
     with pytest.raises(KeyError):
         run_path_integral(PArgs(env_name="car2d", Nsample=64, Nrefine=3, update_method="nope"))
-
-
-@pytest.mark.parametrize("Nn", [2048, 8192])
-def test_single_kernel_step_equals_separate_launches(humanoidrun_setup, Nn):
-    """mbd_reverse_step (ONE cooperative kernel per diffusion step, kept in the ABI) is bit-identical to the separate
-    round-1 kernels it replays (mbd_sample_rollout + mbd_softmax_weights + mbd_weighted_sum_runs + mbd_update)."""
-    env, blob, st = humanoidrun_setup
-    _, alphas, alphas_bar, sigmas = opl.make_schedule(1e-4, 1e-2, 300)
-    coef = eng.update_coef(alphas, alphas_bar, 200)
-    key = np.uint32([8, 9]); Ybar_i = torch.as_tensor((np.random.default_rng(1).normal(size=850) * 0.1).astype(np.float32), device=DEV)
-    m = env.device_model(torch.device(DEV)); sti = torch.as_tensor(st, device=DEV)
-
-    def buffers():
-        return dict(Y=torch.empty((Nn, 850), device=DEV), r=torch.empty(Nn, device=DEV), w=torch.empty(Nn, device=DEV),
-                    sc=torch.zeros(4, device=DEV), runs=torch.empty(((Nn + 63) // 64) * 850, device=DEV), out=torch.empty(850, device=DEV))
-    a, b = buffers(), buffers()
-    ops.sample_rollout(m, sti, key, Nn, 0, Nn, 50, float(sigmas[200]), Ybar_i, a["Y"], a["r"])
-    ops.softmax_weights(a["r"], None, 0, Nn, 0.1, 0.0, a["w"], a["sc"], torch.empty(Nn, device=DEV))
-    ops.update(a["runs"], ops.weighted_sum_runs(a["w"], a["Y"], 850, a["runs"]), 850, Ybar_i, coef, a["out"])
-    assert ops.reverse_step(m, sti, key, Nn, 50, float(sigmas[200]), Ybar_i, 0.1, coef, b["Y"], b["r"], b["w"], b["sc"], b["runs"], b["out"])
-    for k in ("r", "Y", "w", "sc", "out"):
-        assert_bit_exact(N(b[k]), N(a[k]), k)
-
-
-def test_single_kernel_step_reports_unsupported(humanoidrun_setup):
-    """tiny shards (v1 kernel territory) are not covered: the entry point says so instead of running something else"""
-    env, blob, st = humanoidrun_setup
-    m = env.device_model(torch.device(DEV)); sti = torch.as_tensor(st, device=DEV)
-    z = lambda *s: torch.zeros(*s, device=DEV)   # noqa: E731
-    assert not ops.reverse_step(m, sti, np.uint32([1, 2]), 256, 50, 0.5, z(850), 0.1, [1, 1, 1, 1, 1], z(256, 850), z(256), z(256), z(4),
-                                z(4 * 850), z(850))

@@ -15,13 +15,12 @@ DEV = "cuda:0"
 K = 2.0
 HUMANOIDS = ["humanoidrun", "humanoidstandup", "humanoidtrack"]
 OTHERS = ["hopper", "walker2d", "ant", "halfcheetah", "cartpole", "contact_params"] + [f"gen{s}" for s in F.MODELGEN_SEEDS]
-CASES = [(m, v) for m in HUMANOIDS for v in (0, 1, 2, 3, 5, 6, 8, 9)] + [(m, v) for m in OTHERS for v in (1, 2)]
+CASES = [(m, v) for m in HUMANOIDS for v in (0, 1, 2, 3, 8)] + [(m, v) for m in OTHERS for v in (1, 2)]
 
 
 def launched_kernel(blob, variant, n, sms):
     """the rollout kernel `launch_rollout` (csrc/mbd_b200.cu) runs for a requested variant: it remaps variants a model cannot
-    take (named barriers need 2 per parent within 15, the packed kernel needs 11 hinge-only links, the two-group CTA at most
-    2 contacts per link)"""
+    take (named barriers need 2 per parent within 15, the packed kernel 11 hinge-only links with at most 2 contacts each)"""
     bi = blob.view(np.int32)
     L = int(bi[B.H_NLINK])
     lf = lambda f: bi[B.HDR_WORDS + f * B.MAXL:B.HDR_WORDS + f * B.MAXL + L]   # noqa: E731
@@ -32,18 +31,14 @@ def launched_kernel(blob, variant, n, sms):
     v = variant
     if v == 0:
         v = (1 if n <= sms * 16 else 3 if n <= sms * 32 else 8 if max_ncon <= 2 and pk_ok else 2) if L == 11 else 2
-    if not named_ok:
-        v = {3: 2, 9: 8}.get(v, v)
-    if v in (8, 9) and not pk_ok:
+    if not named_ok and v == 3:
         v = 2
-    if v in (8, 9):
-        return ("pk-group" if v == 8 else "pk-named") + ("" if max_ncon <= 2 else "-6con")
+    if v == 8 and not (pk_ok and max_ncon <= 2):
+        v = 2
+    if v == 8:
+        return "pk-group"
     if v == 1:
         return "lane-per-link"
-    if v == 5:
-        return "wpl-split2"
-    if L == 11 and v == 6 and max_ncon <= 2:
-        return "wpl-two-groups"
     if L == 11 and v == 2:
         return "wpl-cta"
     if L == 11 and v == 3:
@@ -55,8 +50,7 @@ def test_every_rollout_kernel_is_covered(tmp_path):
     """the (model, variant) cases below launch every rollout kernel at least once, after the launcher's remapping"""
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     got = {launched_kernel(F.make_env(m, tmp_path).blob, v, 129, sms) for m, v in CASES}
-    want = {"lane-per-link", "wpl-cta", "wpl-named", "wpl-split2", "wpl-two-groups", "wpl-generic",
-            "pk-group", "pk-named", "pk-group-6con", "pk-named-6con"}
+    want = {"lane-per-link", "wpl-cta", "wpl-named", "wpl-generic", "pk-group"}
     assert want <= got, want - got
 
 
