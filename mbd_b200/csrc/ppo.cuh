@@ -92,12 +92,14 @@ __global__ void __launch_bounds__(kPpoThreads) k_ppo_act(mbd_ppo_plan p, int mod
   ppo_advance(p.act_ctl_dev, mode);
 }
 
-// running_statistics.update, (1): per chunk of MBD_PPO_STAT_ROWS rows and per column, S1 = sum d and S2 = sum d^2 with d = x - old
-// mean, in float64, rows ascending.  Thread = column.
+// running_statistics.update, (1): per chunk of MBD_PPO_STAT_ROWS rows and per column, S1 = sum d and S2 = sum d^2 with d = x - c,
+// in float64, rows ascending.  The shift c is the batch's first row: a value inside the column's spread, so S2 - S1^2 / n keeps the
+// batch's variance where a shift by the old mean would cancel it away (a column 1e4 from a fresh mean of 0 with a 1e-3 spread).
+// Thread = column.
 __global__ void __launch_bounds__(MBD_PPO_MAX_OBS) k_ppo_stat_partial(mbd_ppo_plan p, int rows) {
   const int j = threadIdx.x, O = p.O;
   if (j >= O) return;
-  const double m = p.stat_dev[1 + j];
+  const double m = (double)p.obs_dev[j];
   const int r0 = blockIdx.x * MBD_PPO_STAT_ROWS;
   const int r1 = min(rows, r0 + MBD_PPO_STAT_ROWS);
   double s1 = 0.0, s2 = 0.0;
@@ -110,10 +112,15 @@ __global__ void __launch_bounds__(MBD_PPO_MAX_OBS) k_ppo_stat_partial(mbd_ppo_pl
   p.stat_scratch_dev[((size_t)blockIdx.x * 2 + 1) * O + j] = s2;
 }
 
-// (2): the chunk sums in chunk order; mean += S1 / count; summed_var += sum d (x - new mean) = S2 - (S1 / count) S1
+// (2): the chunk sums in chunk order give the batch mean c + S1 / n and the batch's summed variance M2 = S2 - (S1 / n) S1; the batch
+// joins the old state by the pairwise combination (Chan, Golub and LeVeque), with delta = batch mean - old mean:
+//   mean += delta n / count;  summed_var += M2 + delta^2 n_old n / count.
+// That equals running_statistics.update's mean + sum (x - mean) / count and summed_var + sum (x - old mean)(x - new mean), and every
+// term of the variance is non-negative.
 __global__ void __launch_bounds__(MBD_PPO_MAX_OBS) k_ppo_stat_final(mbd_ppo_plan p, int rows, int chunks) {
   const int j = threadIdx.x, O = p.O;
-  const double count = p.stat_dev[0] + (double)rows;
+  const double n0 = p.stat_dev[0], n = (double)rows;
+  const double count = n0 + n;
   __syncthreads();   // every thread has read the old count before thread 0 writes the new one
   if (j >= O) return;
   double s1 = 0.0, s2 = 0.0;
@@ -121,9 +128,11 @@ __global__ void __launch_bounds__(MBD_PPO_MAX_OBS) k_ppo_stat_final(mbd_ppo_plan
     s1 = s1 + p.stat_scratch_dev[(size_t)c * 2 * O + j];
     s2 = s2 + p.stat_scratch_dev[((size_t)c * 2 + 1) * O + j];
   }
-  const double mu = s1 / count;
-  const double mean = p.stat_dev[1 + j] + mu;
-  const double var = p.stat_dev[1 + O + j] + (s2 - mu * s1);
+  const double mb = s1 / n;
+  const double m2 = s2 - mb * s1;
+  const double delta = ((double)p.obs_dev[j] + mb) - p.stat_dev[1 + j];
+  const double mean = p.stat_dev[1 + j] + delta * (n / count);
+  const double var = p.stat_dev[1 + O + j] + m2 + delta * delta * (n0 * (n / count));
   const double sd = fmin(fmax(sqrt(var / count), 1e-6), 1e6);
   p.stat_dev[1 + j] = mean;
   p.stat_dev[1 + O + j] = var;

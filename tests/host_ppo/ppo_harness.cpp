@@ -28,6 +28,11 @@ int ppo_act_host(const float* policy, const float* mean, const float* std, const
   }
   return 0;
 }
+// the header's composite functions elementwise (tests/test_fp32_spec.py): fn 0 = mbd_tanhf, 1 = mbd_softplusf, 2 = mbd_swishf
+int ppo_fmap_host(int fn, const float* x, int n, float* out) {
+  for (int i = 0; i < n; ++i) out[i] = fn == 0 ? mbd_tanhf(x[i]) : fn == 1 ? mbd_softplusf(x[i]) : mbd_swishf(x[i]);
+  return 0;
+}
 // eps of env b, component j from the key (the in-kernel sampler)
 int ppo_eps_host(uint32_t k0, uint32_t k1, int B, int nu, int part, float* eps) {
   for (int b = 0; b < B; ++b)

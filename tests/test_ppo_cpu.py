@@ -2,7 +2,8 @@
 include/mbd_ppo.h (built with g++) against float64, the parameter layout, the reference's table and derived counts, the key chain,
 the ABI's refusals and the CLI errors.
 
-Acting bound (host harness against float64, the same eps): |act - act64| <= 4e-6, |raw - raw64| <= 2e-6 (1 + |raw64|) and
+Acting bound (host harness against float64, the same eps): within 2 radii of the float64 contract (tests/rl_ref.py), and
+|act - act64| <= 4e-6, |raw - raw64| <= 2e-6 (1 + |raw64|) and
 |logp - logp64| <= 1e-4 (1 + |logp64|).  The fp32 functions are accurate to a few ulp (tests/test_fp32_spec.py); the sums over up to
 128 inputs and the cancellation in 1 - 2 / (exp(2|x|) + 1) near 0 set the rest."""
 import ctypes
@@ -157,6 +158,13 @@ def test_host_harness_against_float64(harness, O, nu):
     assert np.abs(act - a64).max() <= 4e-6
     assert np.all(np.abs(raw - r64) <= 2e-6 * (1 + np.abs(r64)))
     assert np.all(np.abs(logp - l64) <= 1e-4 * (1 + np.abs(l64)))
+    # the float64 contract (tests/rl_ref.py, DESIGN.md §2): every word within 2 radii of the reference, whose values are
+    # the restatement's
+    from tests import rl_ref
+    b = rl_ref.act("ppo", policy, mean, std, obs, eps, O, nu)
+    for got, want, w64 in ((act, b["act"], a64), (raw, b["raw"], r64), (logp, b["logp"], l64)):
+        np.testing.assert_allclose(want.v, w64, rtol=1e-9, atol=1e-9)
+        assert rl_ref.ratio(got, want).max() <= 2.0
 
 
 @pytest.mark.parametrize("part", [0, 1])

@@ -2,7 +2,8 @@
 ring against Brax's rolling queue, the hopper row's step accounting, the key chain, the torch fp32 losses and one sgd_step against a
 float64 restatement, the ABI's refusals and the CLI errors.
 
-Acting bound (host harness against float64, the same eps): |act - act64| <= 4e-6, |raw - raw64| <= 2e-6 (1 + |raw64|) and
+Acting bound (host harness against float64, the same eps): within 2 radii of the float64 contract (tests/rl_ref.py), and
+|act - act64| <= 4e-6, |raw - raw64| <= 2e-6 (1 + |raw64|) and
 |logp - logp64| <= 1e-4 (1 + |logp64|), the bounds of tests/test_ppo_cpu.py.  The layers are wider here (256 inputs instead of 32)
 but ReLU passes errors through without amplification: with weights of lecun scale a unit's accumulated fp32 error stays below
 ~256 * 2^-24 * sum |x_i w_i|, about 1e-5 relative, and the head's functions are accurate to a few ulp (tests/test_fp32_spec.py).
@@ -75,6 +76,13 @@ def test_host_harness_against_float64(sac_harness, O, nu):
     assert np.abs(act - a64).max() <= 4e-6
     assert np.all(np.abs(raw - r64) <= 2e-6 * (1 + np.abs(r64)))
     assert np.all(np.abs(logp - l64) <= 1e-4 * (1 + np.abs(l64)))
+    # the float64 contract (tests/rl_ref.py, DESIGN.md §2): every word within 2 radii of the reference, whose values are
+    # the restatement's
+    from tests import rl_ref
+    b = rl_ref.act("sac", policy, mean, std, obs, eps, O, nu)
+    for got, want, w64 in ((act, b["act"], a64), (raw, b["raw"], r64), (logp, b["logp"], l64)):
+        np.testing.assert_allclose(want.v, w64, rtol=1e-9, atol=1e-9)
+        assert rl_ref.ratio(got, want).max() <= 2.0
 
 
 def test_hopper_policy_size():
