@@ -429,6 +429,43 @@ int mbd_sac_sample(const mbd_sac_plan* plan, mbd_stream s);
 /* sizeof / offsetof of mbd_sac_plan and the MBD_SAC_* limits (cross-checked against the ctypes mirror) */
 int mbd_sac_abi_sizes(int32_t* out, int n);
 
+/* ---- the fused SAC gradient update (include/mbd_sac_learn.h, csrc/sac_learn.cuh) ---------------------------------------------
+ * One Brax sgd_step on the batch and noise of update g = *upd_ctl_dev (the sampler's batch_dev / eps_dev of mbd_sac_plan): the three
+ * losses with the old parameters, Adam on the policy, Q and log alpha (torch.optim.Adam's formula, the step count ctl_dev[0] + 1),
+ * then target_q += tau (q - target_q).  Two launches, no float atomics, graph-capturable: the second launch's last CTA stores the
+ * step count and g + 1.  A launch with g outside 0 .. updates - 1 changes nothing.  MBD_EINVAL (with mbd_last_error) before any
+ * CUDA call for O outside 1..128, Nu outside 1..32, batch outside 1..MBD_SAC_LEARN_MAX_BATCH, updates < 1, scratch_floats below
+ * mbd_sac_learn_scratch(O, Nu, batch) or a missing buffer. */
+typedef struct mbd_sac_learn_plan {
+  int32_t O, nu, batch, updates;
+  float learning_rate;           /* the policy's and Q's Adam rate (log alpha: 3e-4) */
+  float reward_scaling, discounting, tau;
+  float* policy_dev;             /* flat policy (include/mbd_sac.h), updated in place */
+  float* q_dev;                  /* layer-major two-critic Q (mbd_b200/rl/networks.py) */
+  float* target_q_dev;
+  float* log_alpha_dev;          /* [1] */
+  float* policy_m_dev;           /* Adam moments, the layouts of their parameters */
+  float* policy_v_dev;
+  float* q_m_dev;
+  float* q_v_dev;
+  float* alpha_mv_dev;           /* [2]: log alpha's m, v */
+  int64_t* ctl_dev;              /* [2]: the Adam step count (updates done), ticket (0) */
+  const float* mean_dev;         /* [O] observation statistics */
+  const float* std_dev;
+  const float* batch_dev;        /* [updates][batch][mbd_sac_row(O, Nu)] */
+  const float* eps_dev;          /* [3][updates][batch][Nu]: the noise of the alpha, critic and actor losses */
+  int64_t* upd_ctl_dev;          /* [1] the update of the training step */
+  float* scratch_dev;            /* mbd_sac_learn_scratch(O, Nu, batch) floats */
+  int64_t scratch_floats;
+  float* losses_dev;             /* [3]: alpha, critic and actor loss of the last update */
+} mbd_sac_learn_plan;
+/* floats of the scratch buffer of one update */
+int64_t mbd_sac_learn_scratch(int O, int nu, int batch);
+/* one sgd_step (two launches) */
+int mbd_sac_update(const mbd_sac_learn_plan* plan, mbd_stream s);
+/* sizeof / offsetof of mbd_sac_learn_plan and the limits (cross-checked against the ctypes mirror) */
+int mbd_sac_learn_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

@@ -95,10 +95,21 @@ class SacPlan(ctypes.Structure):
                 ("eps_dev", c_vp)]
 
 
+class SacLearnPlan(ctypes.Structure):
+    """mbd_sac_learn_plan (include/mbd_b200.h): the fused SAC gradient update"""
+    _fields_ = [("O", ctypes.c_int32), ("nu", ctypes.c_int32), ("batch", ctypes.c_int32), ("updates", ctypes.c_int32),
+                ("learning_rate", ctypes.c_float), ("reward_scaling", ctypes.c_float), ("discounting", ctypes.c_float),
+                ("tau", ctypes.c_float), ("policy_dev", c_vp), ("q_dev", c_vp), ("target_q_dev", c_vp), ("log_alpha_dev", c_vp),
+                ("policy_m_dev", c_vp), ("policy_v_dev", c_vp), ("q_m_dev", c_vp), ("q_v_dev", c_vp), ("alpha_mv_dev", c_vp),
+                ("ctl_dev", c_vp), ("mean_dev", c_vp), ("std_dev", c_vp), ("batch_dev", c_vp), ("eps_dev", c_vp),
+                ("upd_ctl_dev", c_vp), ("scratch_dev", c_vp), ("scratch_floats", ctypes.c_int64), ("losses_dev", c_vp)]
+
+
 PPO_ACT, PPO_RECORD, PPO_EVAL, PPO_EVAL_RECORD = 0, 1, 2, 3   # MBD_PPO_*
 PPO_MAX_OBS, PPO_MAX_NU, PPO_MAX_MB, PPO_STAT_ROWS = 128, 32, 4096, 256
 SAC_ACT, SAC_EVAL, SAC_EVAL_RECORD = 0, 1, 2                   # MBD_SAC_*
 SAC_MAX_CAPACITY, SAC_HIDDEN = 1 << 24, 256
+SAC_LEARN_MAX_BATCH = 4096                                     # MBD_SAC_LEARN_MAX_BATCH
 
 VEC_XPBD, VEC_CAR2D, VEC_PUSHT = 0, 1, 2                                   # MBD_VEC_*
 VEC_OBS = {"qqd": 0, "hopper": 1, "skip2": 2, "skip1": 3, "state": 4}     # MBD_VEC_OBS_*
@@ -182,6 +193,10 @@ def lib():
     L.mbd_sac_record.argtypes = [ctypes.POINTER(SacPlan), c_vp]
     L.mbd_sac_sample.argtypes = [ctypes.POINTER(SacPlan), c_vp]
     L.mbd_sac_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_sac_learn_scratch.restype = ctypes.c_int64
+    L.mbd_sac_learn_scratch.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    L.mbd_sac_update.argtypes = [ctypes.POINTER(SacLearnPlan), c_vp]
+    L.mbd_sac_learn_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes = [ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -196,7 +211,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

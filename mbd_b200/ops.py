@@ -287,6 +287,17 @@ def sac_sample(plan: "_lib.SacPlan"):
     check(_lib.lib().mbd_sac_sample(ctypes.byref(plan), _stream()), "mbd_sac_sample")
 
 
+def sac_learn_scratch(O: int, nu: int, batch: int) -> int:
+    """floats of the fused SAC update's scratch buffer (mbd_sac_learn_scratch)"""
+    return int(_lib.lib().mbd_sac_learn_scratch(int(O), int(nu), int(batch)))
+
+
+def sac_update(plan: "_lib.SacLearnPlan"):
+    """one fused SAC gradient update (mbd_sac_update: two launches): the three losses, Adam on the policy, Q and log alpha, the
+    Polyak step, then the update counter advances"""
+    check(_lib.lib().mbd_sac_update(ctypes.byref(plan), _stream()), "mbd_sac_update")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

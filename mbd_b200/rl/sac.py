@@ -3,7 +3,8 @@
 Acting is one CUDA launch per env step (`mbd_sac_act`, csrc/sac.cuh) followed by the two launches of the vector env's step, the
 replay record (`mbd_sac_record`) and PPO's observation statistics (`mbd_ppo_obs_stats` over the B acting observations).  The replay
 buffer is a device ring with Brax's queue semantics, and one `mbd_sac_sample` launch per training step draws the batch of every
-gradient update and the noise of its three losses.  The losses and the three Adam optimisers are torch fp32.  Every key of a run is
+gradient update and the noise of its three losses.  The losses and the three Adam optimisers are torch fp32 (`Learner`, the
+default) or two CUDA launches per update (`FusedLearner`, learner="fused").  Every key of a run is
 computed on the host up front (`key_chain`) and read on the device through counters: a training step is the acting graph, the
 sampling graph and 64 replays of the update graph, with no host synchronisation.
 
@@ -192,6 +193,68 @@ class Learner:
                                                                        for st in o.state.values() for s in st.values()]
 
 
+class FusedLearner:
+    """The same sgd_step as `Learner` as two CUDA launches (mbd_sac_update, include/mbd_sac_learn.h): the three losses with the old
+    parameters, the three Adam steps and the Polyak step.  The parameters, the Adam moments and the step count live on the device;
+    the policy is updated in place, so an acting plan that holds its pointer sees every update.  `bind` points the learner at the
+    sampler's batch [updates, batch, row] and noise [3, updates, batch, Nu] buffers, the update counter (int64 [1]) and the
+    observation statistics; each `update()` then runs update *upd_ctl and advances it."""
+
+    def __init__(self, policy: np.ndarray, q: np.ndarray, O: int, nu: int, learning_rate: float, reward_scaling: float,
+                 discounting: float, tau: float, device, batch_size: int):
+        d = torch.device(device)
+        if d.type != "cuda":
+            raise ValueError("the fused learner runs on a CUDA device")
+        if not 1 <= batch_size <= _lib.SAC_LEARN_MAX_BATCH:
+            raise ValueError(f"batch_size must be in 1..{_lib.SAC_LEARN_MAX_BATCH}")
+        self.O, self.nu, self.batch_size = O, nu, batch_size
+        self.learning_rate, self.reward_scaling, self.discounting, self.tau = learning_rate, reward_scaling, discounting, tau
+        f32 = dict(device=d, dtype=torch.float32)
+        self.policy = torch.tensor(np.asarray(policy, np.float32), device=d)
+        self.q = torch.tensor(np.asarray(q, np.float32), device=d)
+        self.target_q = self.q.clone()
+        self.log_alpha = torch.zeros(1, **f32)
+        self.policy_m, self.policy_v = torch.zeros_like(self.policy), torch.zeros_like(self.policy)
+        self.q_m, self.q_v = torch.zeros_like(self.q), torch.zeros_like(self.q)
+        self.alpha_mv = torch.zeros(2, **f32)
+        self.ctl = torch.zeros(2, device=d, dtype=torch.int64)     # Adam step count, ticket
+        self.losses = torch.zeros(3, **f32)                         # alpha, critic, actor loss of the last update
+        self.scratch = torch.zeros(ops.sac_learn_scratch(O, nu, batch_size), **f32)
+        self.plan = None
+
+    def bind(self, batch: torch.Tensor, eps: torch.Tensor, upd_ctl: torch.Tensor, mean: torch.Tensor, std: torch.Tensor):
+        G = batch.shape[0]
+        if tuple(batch.shape) != (G, self.batch_size, 2 * self.O + self.nu + 3) or tuple(eps.shape) != (3, G, self.batch_size, self.nu):
+            raise ValueError("batch must be [updates, batch_size, row] and eps [3, updates, batch_size, nu]")
+        if upd_ctl.dtype != torch.int64 or upd_ctl.numel() < 1:
+            raise ValueError("upd_ctl must be an int64 tensor")
+        self._bound = (batch, eps, upd_ctl, mean, std)      # keeps the buffers alive as long as the plan points at them
+        P = _lib.SacLearnPlan()
+        P.O, P.nu, P.batch, P.updates = self.O, self.nu, self.batch_size, G
+        P.learning_rate, P.reward_scaling, P.discounting, P.tau = self.learning_rate, self.reward_scaling, self.discounting, self.tau
+        P.policy_dev, P.q_dev, P.target_q_dev, P.log_alpha_dev = (t.data_ptr() for t in (self.policy, self.q, self.target_q,
+                                                                                         self.log_alpha))
+        P.policy_m_dev, P.policy_v_dev, P.q_m_dev, P.q_v_dev, P.alpha_mv_dev = (t.data_ptr() for t in (
+            self.policy_m, self.policy_v, self.q_m, self.q_v, self.alpha_mv))
+        P.ctl_dev, P.mean_dev, P.std_dev = self.ctl.data_ptr(), mean.data_ptr(), std.data_ptr()
+        P.batch_dev, P.eps_dev, P.upd_ctl_dev = batch.data_ptr(), eps.data_ptr(), upd_ctl.data_ptr()
+        P.scratch_dev, P.scratch_floats, P.losses_dev = self.scratch.data_ptr(), self.scratch.numel(), self.losses.data_ptr()
+        self.plan = P
+
+    def update(self):
+        if self.plan is None:
+            raise RuntimeError("bind the learner to its batch, noise and counter first")
+        with torch.cuda.device(self.policy.device):
+            ops.sac_update(self.plan)
+
+    def state(self):
+        return [self.policy, self.q, self.target_q, self.log_alpha, self.policy_m, self.policy_v, self.q_m, self.q_v, self.alpha_mv,
+                self.ctl]
+
+
+LEARNERS = ("torch", "fused")
+
+
 # ---- acting ------------------------------------------------------------------------------------------------------------------------
 class Actor:
     """The stochastic SAC policy on a VecEnv, with ppo.Actor's protocol: `act(key)` writes tanh(raw) for every env into the VecEnv's
@@ -240,7 +303,11 @@ class Actor:
 class SACTrainer:
     def __init__(self, env, num_timesteps: int, episode_length: int, num_envs: int, num_eval_envs: int, learning_rate: float,
                  discounting: float, seed: int, batch_size: int, num_evals: int, normalize_observations: bool, reward_scaling: float,
-                 tau: float, min_replay_size: int, max_replay_size: int, grad_updates_per_step: int, device=None):
+                 tau: float, min_replay_size: int, max_replay_size: int, grad_updates_per_step: int, device=None,
+                 learner: str = "torch"):
+        if learner not in LEARNERS:
+            raise ValueError(f"learner must be one of {LEARNERS}, not {learner!r}")
+        self.learner_kind = learner
         _lib.require_gpu()
         if not num_envs <= max_replay_size <= _lib.SAC_MAX_CAPACITY:
             raise ValueError(f"max_replay_size must be in num_envs..{_lib.SAC_MAX_CAPACITY}")
@@ -261,8 +328,12 @@ class SACTrainer:
             raise ValueError(f"observation size {O} / action size {nu} above {_lib.PPO_MAX_OBS} / {_lib.PPO_MAX_NU}")
         self.O, self.nu, self.R = O, nu, 2 * O + nu + 3
         psizes, qsizes = nets.sac_policy_sizes(O, nu), nets.sac_q_sizes(O, nu)
-        self.learner = Learner(nets.init_params(K.policy, psizes), nets.sac_q_init(K.q, qsizes), O, nu, learning_rate, reward_scaling,
-                               discounting, tau, d)
+        if self.learner_kind == "fused":
+            self.learner = FusedLearner(nets.init_params(K.policy, psizes), nets.sac_q_init(K.q, qsizes), O, nu, learning_rate,
+                                        reward_scaling, discounting, tau, d, mb)
+        else:
+            self.learner = Learner(nets.init_params(K.policy, psizes), nets.sac_q_init(K.q, qsizes), O, nu, learning_rate,
+                                   reward_scaling, discounting, tau, d)
         f32 = dict(device=d, dtype=torch.float32)
         self.mean, self.std = torch.zeros(O, **f32), torch.ones(O, **f32)
         self.stat = torch.zeros(1 + 2 * O, device=d, dtype=torch.float64)
@@ -279,6 +350,8 @@ class SACTrainer:
         self.batch = torch.zeros((G, mb, self.R), **f32)
         self.eps = torch.zeros((3, G, mb, nu), **f32)
         self.upd_ctl = torch.zeros(1, device=d, dtype=torch.int64)
+        if self.learner_kind == "fused":
+            self.learner.bind(self.batch, self.eps, self.upd_ctl, self.mean, self.std)
         v = self.venv
         P = _lib.SacPlan()
         P.B, P.O, P.nu, P.capacity, P.batch, P.updates = B, O, nu, self.cap, mb, G
@@ -319,6 +392,9 @@ class SACTrainer:
 
     def sgd_step(self):
         """update upd_ctl of the training step: its batch and noise, Brax's sgd_step, then upd_ctl += 1"""
+        if self.learner_kind == "fused":
+            self.learner.update()         # reads the batch and noise at upd_ctl and advances it on the device
+            return
         with torch.no_grad():
             rows = torch.index_select(self.batch.view(self.G, -1), 0, self.upd_ctl).view(self.mb, self.R)
             eps = torch.index_select(self.eps.view(3, self.G, -1), 1, self.upd_ctl).view(3, self.mb, self.nu)
@@ -333,8 +409,9 @@ class SACTrainer:
                 self._act_graph.replay() if self._act_graph is not None else self.actor_step()
 
     def capture(self):
-        """captures the acting step, the sampling and one update as CUDA graphs (and the evaluation step).  The update is warmed up
-        on a side stream first and every state it touched is restored, so capturing changes no result."""
+        """captures the acting step, the sampling and one update as CUDA graphs (and the evaluation step).  The torch update is
+        warmed up on a side stream first and every state it touched is restored, so capturing changes no result; the fused update is
+        two kernel launches and is captured without running."""
         with torch.cuda.device(self.dev):
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
@@ -344,22 +421,8 @@ class SACTrainer:
             with torch.cuda.graph(g):
                 self.sample()
             self._sample_graph = g
-            L = self.learner
-            kept = (L.policy, L.q, L.target_q, L.log_alpha, self.upd_ctl)
-            snap = [t.detach().clone() for t in kept]
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                for _ in range(2):
-                    self.sgd_step()
-            torch.cuda.current_stream().wait_stream(s)
-            with torch.no_grad():
-                for t, v in zip(kept, snap):
-                    t.copy_(v)
-                for t in L.state()[4:]:     # the optimisers' moments and step counts
-                    t.zero_()
-                for t in (L.policy.grad, L.q.grad, L.log_alpha.grad):
-                    t.zero_()
+            if self.learner_kind == "torch":
+                self._warm_torch_update()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self.sgd_step()
@@ -369,6 +432,25 @@ class SACTrainer:
                 self.actor.act()
                 ops.vec_step(self.evenv.plan)
             self._eval_graph = g
+
+    def _warm_torch_update(self):
+        """two torch updates on a side stream (the optimisers allocate their state), then every state they touched restored"""
+        L = self.learner
+        kept = (L.policy, L.q, L.target_q, L.log_alpha, self.upd_ctl)
+        snap = [t.detach().clone() for t in kept]
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            for _ in range(2):
+                self.sgd_step()
+        torch.cuda.current_stream().wait_stream(s)
+        with torch.no_grad():
+            for t, v in zip(kept, snap):
+                t.copy_(v)
+            for t in L.state()[4:]:     # the optimisers' moments and step counts
+                t.zero_()
+            for t in (L.policy.grad, L.q.grad, L.log_alpha.grad):
+                t.zero_()
 
     def training_step(self):
         """Brax's training_step: an actor step, the replay sample, grad_updates_per_step updates"""
@@ -413,10 +495,14 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
           learning_rate: float = 1e-4, discounting: float = 0.9, seed: int = 0, batch_size: int = 256, num_evals: int = 1,
           normalize_observations: bool = False, max_devices_per_host: Optional[int] = None, reward_scaling: float = 1.0,
           tau: float = 0.005, min_replay_size: int = 0, max_replay_size: Optional[int] = None, grad_updates_per_step: int = 1,
-          deterministic_eval: bool = False, progress_fn: Callable[[int, dict], None] = lambda *a: None, capture: bool = True):
+          deterministic_eval: bool = False, progress_fn: Callable[[int, dict], None] = lambda *a: None, capture: bool = True,
+          learner: str = "torch"):
     """sac.train with Brax's signature and defaults for the arguments the reference passes.  Returns (make_inference_fn, params,
     metrics): make_inference_fn(params) gives an `Actor` factory for a VecEnv; params is a dict of numpy arrays (policy, q, target_q,
-    log_alpha, the observation statistics).  One device: max_devices_per_host is accepted and has nothing to choose."""
+    log_alpha, the observation statistics).  One device: max_devices_per_host is accepted and has nothing to choose.  learner:
+    "torch" (`Learner`, the default) or "fused" (`FusedLearner`, the update as two CUDA launches)."""
+    if learner not in LEARNERS:
+        raise ValueError(f"learner must be one of {LEARNERS}, not {learner!r}")
     if action_repeat != 1:
         raise NotImplementedError("action_repeat != 1 is not built (the vector env steps once per action)")
     if deterministic_eval:
@@ -425,7 +511,8 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
         max_replay_size = num_timesteps
     env = get_env(environment) if isinstance(environment, str) else environment
     tr = SACTrainer(env, num_timesteps, episode_length, num_envs, num_eval_envs, learning_rate, discounting, seed, batch_size, num_evals,
-                    normalize_observations, reward_scaling, tau, min_replay_size, max_replay_size, grad_updates_per_step)
+                    normalize_observations, reward_scaling, tau, min_replay_size, max_replay_size, grad_updates_per_step,
+                    learner=learner)
     if capture:
         tr.capture()
     c = tr.c

@@ -2,7 +2,8 @@
 
 Trains SAC (mbd_b200.rl.sac) with the reference's hopper hyperparameters and then runs the same tail as train_brax: the
 `step: N, episode return: X` lines, `time to jit`, `time to train`, results/{env}/params.npz, the mean reward of 8 episodes of 50
-steps and results/{env}/RL.html.  --num_timesteps and --seed override the table for short runs.  The PPO envs are trained by
+steps and results/{env}/RL.html.  --num_timesteps and --seed override the table for short runs; --learner fused runs the gradient
+update as the fused CUDA kernels (sac.FusedLearner) instead of the torch learner.  The PPO envs are trained by
 python -m mbd_b200.rl.train_brax.
 """
 from __future__ import annotations
@@ -26,6 +27,8 @@ def main(argv=None):
     ap.add_argument("--env_name", default="hopper")
     ap.add_argument("--num_timesteps", type=int, default=None, help="override the table's num_timesteps")
     ap.add_argument("--seed", type=int, default=None, help="override the table's seed")
+    ap.add_argument("--learner", default="torch", choices=("torch", "fused"),
+                    help="the gradient update: torch ops (default) or the fused CUDA update")
     a = ap.parse_args(argv)
     if a.env_name not in SAC_TABLE:
         raise SystemExit(f"{a.env_name}: the reference trains it with Brax PPO: run python -m mbd_b200.rl.train_brax --env_name {a.env_name}")
@@ -41,7 +44,7 @@ def main(argv=None):
     if a.seed is not None:
         cfg["seed"] = a.seed
     progress, times = progress_printer()
-    make_inference_fn, params, _ = sac.train(environment=env, progress_fn=progress, **cfg)
+    make_inference_fn, params, _ = sac.train(environment=env, progress_fn=progress, learner=a.learner, **cfg)
     post_training(a.env_name, env, make_inference_fn, params, times)
 
 
