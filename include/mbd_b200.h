@@ -65,6 +65,13 @@ int mbd_rollout(const mbd_model* m, const float* state_init_dev, const float* Y0
                 float* rewss_dev, float* rews_dev, const float* xref_dev, int href, float* logpd_dev,
                 float* final_state_dev, float* track_pos_dev, int nsub_override, mbd_stream s);
 
+/* mbd_rollout that also records the rollout: traj_dev [n,H,L,13] receives every link's state after each of the H env steps
+ * (the layout of final_state_dev, once per step; row H-1 equals final_state_dev).  It runs the warp-per-link kernel whatever n is;
+ * every output is bit-identical to mbd_rollout's.  traj_dev == NULL is exactly mbd_rollout. */
+int mbd_rollout_traj(const mbd_model* m, const float* state_init_dev, const float* Y0s_dev, int n, int H,
+                     float* rewss_dev, float* rews_dev, const float* xref_dev, int href, float* logpd_dev,
+                     float* final_state_dev, float* track_pos_dev, int nsub_override, float* traj_dev, mbd_stream s);
+
 /* mbd_sample + mbd_rollout fused in ONE kernel (each CTA draws the noise of its own samples,
  * writes Y0s once, then rolls them out): the hot path of reverse_once, mbd_planner.py:103-110. */
 int mbd_sample_rollout(const mbd_model* m, const float* state_init_dev, const uint32_t key[2], int n_total,

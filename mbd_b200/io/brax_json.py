@@ -51,9 +51,8 @@ def _tolist(a):
     return np.asarray(a, dtype=np.float64).round(6).tolist()
 
 
-def to_dict(sys, pipeline_states: Sequence, dt: float) -> dict:
-    """the document of `brax.io.json.dumps(sys.tree_replace({"opt.timestep": env.dt}), rollout)`"""
-    bs = BraxLikeSystem(sys, dt)
+def _link_geoms(bs: BraxLikeSystem):
+    """-> (link names + "world", {link name: [geom dict]}): the geoms of the document, keyed by the name of their link"""
     link_names = [n or f"link {i}" for i, n in enumerate(bs.link_names)] + ["world"]
     link_geoms = {}
     for i in range(bs.ngeom):
@@ -61,6 +60,13 @@ def to_dict(sys, pipeline_states: Sequence, dt: float) -> dict:
         geom = {"name": GEOM_TYPE_NAMES[int(bs.geom_type[i])], "link_idx": link_idx, "pos": _tolist(bs.geom_pos[i]),
                 "rot": _tolist(bs.geom_quat[i]), "rgba": _tolist(bs.geom_rgba[i]), "size": _tolist(bs.geom_size[i])}
         link_geoms.setdefault(link_names[link_idx], []).append(geom)
+    return link_names, link_geoms
+
+
+def to_dict(sys, pipeline_states: Sequence, dt: float) -> dict:
+    """the document of `brax.io.json.dumps(sys.tree_replace({"opt.timestep": env.dt}), rollout)`"""
+    bs = BraxLikeSystem(sys, dt)
+    link_names, link_geoms = _link_geoms(bs)
     pos = np.stack([np.asarray(ps.x.pos, np.float32) for ps in pipeline_states])
     rot = np.stack([np.asarray(ps.x.rot, np.float32) for ps in pipeline_states])
     return {"link_names": link_names[:-1], "opt": {"timestep": float(dt)}, "dt": float(dt), "geoms": link_geoms,
@@ -71,12 +77,63 @@ def dumps(sys, pipeline_states: Sequence, dt: float) -> str:
     return json.dumps(to_dict(sys, pipeline_states, dt))
 
 
-def render(sys, pipeline_states: Sequence, dt: float, height: int = 480) -> str:
-    """the page `brax.io.html.render` returns: the JSON document embedded next to the Brax viewer module"""
-    doc = dumps(sys, pipeline_states, dt)
+def diffusion_to_dict(sys, pos, rot, dt: float, lift: bool = False) -> dict:
+    """the document of `dumps` in the reference's scripts/vis_diffusion.py:27-112, from the world poses pos [K,T,L,3], rot [K,T,L,4]
+    of K rollouts of T steps (one per diffusion iterate, the state before each step).
+
+    Every link is drawn T times, copy k named `{name}_{k}` (k = 0 keeps the plain name) with its link_idx offset by k * L, so that
+    one frame shows all T poses of a rollout.  Colours: world geoms as they are; `goal` links green (not offset: every copy sits on
+    copy 0's pose); `_ref` links (humanoidtrack's reference bodies) torso / thigh fading green, the rest invisible; every other link
+    fading red, from pale at k = 0 to full at k = T - 1.  Frames: one per rollout, then T frames that play the last rollout with
+    every copy on that step's pose.  lift (pushT): step i is raised by i * 0.01 / 50 so that the copies do not overlap."""
+    bs = BraxLikeSystem(sys, dt)
+    link_names, link_geoms = _link_geoms(bs)
+    pos, rot = np.asarray(pos, np.float32), np.asarray(rot, np.float32)
+    K, T, L = pos.shape[:3]
+    nl = len(link_names) - 1
+    all_link_geoms, all_link_names = {}, []
+    for k in range(T):
+        a = k / T * 0.8 + 0.2
+        for name, geoms in link_geoms.items():
+            name = f"{name}_{k}" if k > 0 else name
+            geoms_new = []
+            for geom in geoms:
+                g = dict(geom)
+                if "world" in name:
+                    g["link_idx"] = -1
+                elif "goal" in name:
+                    g["rgba"] = [0.0, 1.0, 0.0, 1.0]
+                elif "_ref" in name:
+                    if "torso" in name or "thigh" in name:
+                        g["link_idx"] = geom["link_idx"] + k * nl
+                        g["rgba"] = [1 - a, 1.0, 1 - a, 1.0]
+                    else:
+                        g["rgba"] = [1.0, 1.0, 1.0, 0.0]
+                else:
+                    g["link_idx"] = geom["link_idx"] + k * nl
+                    g["rgba"] = [1.0, 1 - a, 1 - a, 1.0]
+                geoms_new.append(g)
+            all_link_geoms[name] = geoms_new
+            all_link_names.append(name)
+    if lift:
+        z = np.float32([i * 0.01 / 50 for i in range(T)])
+        pos = pos + np.stack([np.zeros_like(z), np.zeros_like(z), z], axis=-1)[None, :, None, :]
+    fpos = np.concatenate([pos.reshape(K, T * L, 3), np.tile(pos[-1][:, None], (1, T, 1, 1)).reshape(T, T * L, 3)])
+    frot = np.concatenate([rot.reshape(K, T * L, 4), np.tile(rot[-1][:, None], (1, T, 1, 1)).reshape(T, T * L, 4)])
+    return {"link_names": all_link_names, "opt": {"timestep": float(dt)}, "dt": float(dt), "geoms": all_link_geoms,
+            "states": {"x": {"pos": _tolist(fpos), "rot": _tolist(frot)}}}
+
+
+def page(doc: str, height: int = 480) -> str:
+    """the page `brax.io.html.render_from_json` returns: the JSON document embedded next to the Brax viewer module"""
     return ("<html><head><title>brax visualizer</title><style>body{margin:0;padding:0;}#brax-viewer{margin:0;padding:0;height:"
             f"{int(height)}px;}}</style></head><body><script type=\"application/javascript\">var system = {doc};</script>"
             "<div id=\"brax-viewer\"></div><script type=\"module\">"
             f"import {{Viewer}} from '{VIEWER_JS}';"
             "const domElement = document.getElementById('brax-viewer');var viewer = new Viewer(domElement, system);"
             "</script></body></html>")
+
+
+def render(sys, pipeline_states: Sequence, dt: float, height: int = 480) -> str:
+    """the page `brax.io.html.render` returns: the JSON document embedded next to the Brax viewer module"""
+    return page(dumps(sys, pipeline_states, dt), height)

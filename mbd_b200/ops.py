@@ -79,8 +79,9 @@ def sample(key, n_total: int, n_begin: int, n_local: int, HNu: int, sigma: float
 
 
 def rollout(model: Model, state_init: torch.Tensor, Y0s: torch.Tensor, xref: Optional[torch.Tensor] = None,
-            want_rewss=False, want_final=False, want_track=False, nsub_override: int = 0):
-    """vmap(rollout_us)(state_init, Y0s): Y0s [n,H,nu] -> dict(rews [n], rewss, logpd, final, track)."""
+            want_rewss=False, want_final=False, want_track=False, nsub_override: int = 0, want_traj=False):
+    """vmap(rollout_us)(state_init, Y0s): Y0s [n,H,nu] -> dict(rews [n], rewss, logpd, final, track, traj).
+    want_traj: traj [n,H,L,13], every link's raw state after each step (mbd_rollout_traj, the warp-per-link kernel)."""
     state_init, Y0s = _dev(state_init), _dev(Y0s)
     n, H, nu = Y0s.shape
     if nu != model.nu or state_init.numel() != model.L * 13:
@@ -95,9 +96,10 @@ def rollout(model: Model, state_init: torch.Tensor, Y0s: torch.Tensor, xref: Opt
         xref = _dev(xref)
         href = xref.shape[1]
         logpd = torch.empty(n, device=dev)
-    check(_lib.lib().mbd_rollout(model.handle, _p(state_init), _p(Y0s), n, H, _p(rewss), _p(rews), _p(xref), href, _p(logpd),
-                                 _p(final), _p(track), nsub_override, _stream()), "mbd_rollout")
-    return dict(rews=rews, rewss=rewss, logpd=logpd, final=final, track=track)
+    traj = torch.empty((n, H, model.L, 13), device=dev) if want_traj else None
+    check(_lib.lib().mbd_rollout_traj(model.handle, _p(state_init), _p(Y0s), n, H, _p(rewss), _p(rews), _p(xref), href, _p(logpd),
+                                      _p(final), _p(track), nsub_override, _p(traj), _stream()), "mbd_rollout_traj")
+    return dict(rews=rews, rewss=rewss, logpd=logpd, final=final, track=track, traj=traj)
 
 
 def sample_rollout(model: Model, state_init, key, n_total, n_begin, n_local, H, sigma, Ybar, Y0s_out, rews_out,
