@@ -473,6 +473,40 @@ int mbd_sac_update(const mbd_sac_learn_plan* plan, mbd_stream s);
 /* sizeof / offsetof of mbd_sac_learn_plan and the limits (cross-checked against the ctypes mirror) */
 int mbd_sac_learn_abi_sizes(int32_t* out, int n);
 
+/* ---- model-based diffusion as a receding-horizon controller (mbd_b200/planners/mbd_mpc.py, DESIGN.md §5i) ----------------------
+ * B closed loops of one env and shape, each planning with the buffers of mbd_batch_step_launch (params [B][Ndiffuse], ctl [B],
+ * Ybars [B][Ndiffuse][H*nu], rew_hist [B][Ndiffuse]) from the vector env's state (mbd_vec_plan.state_dev, passed as the step plan's
+ * state_init).  mpc_ctl_dev [B] holds the control step c of every problem (zeroed by the caller).  One launch, one CTA per problem,
+ * graph-capturable.  MBD_EINVAL (with mbd_last_error) before any CUDA call for an unknown mode, B outside 1..MBD_VEC_MAX_B, H or nu
+ * below 1, H * nu above 27 * 256, Ndiffuse < 2, Nwarm outside 1..Ndiffuse - 1, Nstep < 1, state_words < 1 or a missing buffer. */
+enum { MBD_MPC_ACT = 0,     /* after control step c's last diffusion step: a_c = Ybars[b][0] row 0 into env_actions and actions[c];
+                             * s_c into states[0] when c = 0; rew_hist[b][1] into rew_hist_log[c]; when c + 1 < Nstep: shift(P_c) into
+                             * Ybars[b][Nwarm], keys row c + 1 into params[b][1 .. Nwarm].key, ctl.i = Nwarm; then c += 1.
+                             * Nothing when c >= Nstep. */
+       MBD_MPC_RECORD = 1 };/* after mbd_vec_step: the env's reward into rewards[c - 1], its state into states[c] (1 <= c <= Nstep) */
+typedef struct mbd_mpc_plan {
+  int32_t B, H, nu;                /* problems, horizon, action size */
+  int32_t Ndiffuse, Nwarm, Nstep;  /* schedule rows, diffusion steps per warm control step, control steps */
+  int32_t state_words;             /* S: words of one env state (the vector env's layout) */
+  int32_t pad;
+  mbd_step_params* params_dev;     /* [B][Ndiffuse] */
+  mbd_step_ctl* ctl_dev;           /* [B] */
+  float* Ybars_dev;                /* [B][Ndiffuse][H*nu] */
+  const float* rew_hist_dev;       /* [B][Ndiffuse] */
+  const uint32_t* keys_dev;        /* [B][Nstep][Nwarm][2]: row c = the keys of diffusion steps 1 .. Nwarm of control step c */
+  int32_t* mpc_ctl_dev;            /* [B] */
+  float* env_actions_dev;          /* the vector env's actions [B][nu], state [B][S] and reward [B] */
+  const float* env_state_dev;
+  const float* env_reward_dev;
+  float* actions_dev;              /* [B][Nstep][nu] executed actions */
+  float* rewards_dev;              /* [B][Nstep] */
+  float* states_dev;               /* [B][Nstep + 1][S] */
+  float* rew_hist_log_dev;         /* [B][Nstep]: rews.mean() of every control step's last diffusion step */
+} mbd_mpc_plan;
+int mbd_mpc_advance(const mbd_mpc_plan* plan, int mode, mbd_stream s);
+/* sizeof / offsetof of mbd_mpc_plan (cross-checked against the ctypes mirror) */
+int mbd_mpc_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

@@ -300,6 +300,12 @@ def sac_update(plan: "_lib.SacLearnPlan"):
     check(_lib.lib().mbd_sac_update(ctypes.byref(plan), _stream()), "mbd_sac_update")
 
 
+def mpc_advance(plan: "_lib.MpcPlan", mode: int):
+    """one launch of the receding-horizon controller (mbd_mpc_advance) in mode _lib.MPC_*: ACT executes every problem's plan and
+    re-arms its next control step, RECORD logs the env step's reward and state"""
+    check(_lib.lib().mbd_mpc_advance(ctypes.byref(plan), int(mode), _stream()), "mbd_mpc_advance")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

@@ -320,10 +320,14 @@ class BatchedDiffusionEngine:
     (`mbd_batch_step_launch`) advances all of them.  Problem b has its own initial state, key chain, schedule (beta0 / betaT
     may differ) and temperature; every per-problem device buffer is [B, ...] with problem b's single-solve block at index b.
     The noise of problem b is drawn from its own key with problem-local counters and every reduction order depends on N only,
-    so problem b reproduces the `DiffusionEngine` solve of the same inputs bit for bit.  One GPU (P = 1)."""
+    so problem b reproduces the `DiffusionEngine` solve of the same inputs bit for bit.  One GPU (P = 1).
+
+    state_buffer: an external [B, S] float32 device tensor the steps read the initial states from instead of the engine's own copy
+    of `state_inits` (the receding-horizon controller passes `VecEnv.state`, so every step plans from the plant's current state).
+    Its layout must be the engine's; its content is the caller's (`state_inits` then only fix the layout)."""
 
     def __init__(self, env, Nsample: int, Hsample: int, temps, enable_demo: bool, state_inits, Ndiffuse: int,
-                 device: Optional[torch.device] = None):
+                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None):
         self.env = env
         self.B = len(state_inits)
         if self.B < 1 or len(temps) != self.B:
@@ -339,6 +343,13 @@ class BatchedDiffusionEngine:
         per = [env_tensors(env, s, self.enable_demo, self.device) for s in state_inits]
         self.model, self.params_car, _, self.xref = per[0]              # shared by every problem
         self.state_init = torch.stack([p[2] for p in per]).contiguous()  # [B, state]
+        if state_buffer is not None:
+            want = (self.B, self.state_init[0].numel())
+            if (not state_buffer.is_cuda or state_buffer.device != self.device or state_buffer.dtype != torch.float32
+                    or not state_buffer.is_contiguous() or tuple(state_buffer.shape) != want):
+                raise ValueError(f"state_buffer must be a contiguous float32 tensor of shape {want} on {self.device} (got "
+                                 f"{state_buffer.dtype} {tuple(state_buffer.shape)} on {state_buffer.device})")
+            self.state_init = state_buffer
         self.rew_xref = float(getattr(env, "rew_xref", 0.0))
         self._alloc(temps)
 
