@@ -507,6 +507,24 @@ int mbd_mpc_advance(const mbd_mpc_plan* plan, int mode, mbd_stream s);
 /* sizeof / offsetof of mbd_mpc_plan (cross-checked against the ctypes mirror) */
 int mbd_mpc_abi_sizes(int32_t* out, int n);
 
+/* ---- the path-integral baselines as receding-horizon controllers (mbd_b200/planners/pi_mpc.py, DESIGN.md §5j) -------------------
+ * The same launch for B closed loops that plan with mbd_pi_batch_step_launch: base is the plan above with the baseline engine's
+ * buffers (Ndiffuse = Nrefine).  The baselines read their sampling sigma from params[b][t].sigma and CMA-ES rewrites it, so ACT
+ * does two more things: it stores params[b][0].sigma, the sigma control step c ended with, into sigma_log[b][c], and when
+ * c + 1 < Nstep it writes sigma_warm into params[b][0 .. Nwarm].sigma, so every warm control step restarts from sigma_warm (a
+ * reset, not a carry; row 0 is never sampled from, it only feeds the log of the methods that leave sigma alone).  RECORD is
+ * mbd_mpc_advance's.  Refuses with MBD_EINVAL (and mbd_last_error) before any CUDA call everything mbd_mpc_advance refuses, a
+ * sigma_warm that is <= 0, NaN or infinite, and in ACT mode a missing sigma_log_dev. */
+typedef struct mbd_mpc_pi_plan {
+  mbd_mpc_plan base;
+  float sigma_warm;                /* the sigma every control step c >= 1 starts from */
+  int32_t pad;
+  float* sigma_log_dev;            /* [B][Nstep] */
+} mbd_mpc_pi_plan;
+int mbd_mpc_pi_advance(const mbd_mpc_pi_plan* plan, int mode, mbd_stream s);
+/* sizeof / offsetof of mbd_mpc_pi_plan (cross-checked against the ctypes mirror) */
+int mbd_mpc_pi_abi_sizes(int32_t* out, int n);
+
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as
  * mbd_step_launch (H*Nu above 27*256 is MBD_EINVAL), except that state_init_dev and the env fields are not read. */

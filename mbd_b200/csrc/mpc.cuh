@@ -1,13 +1,16 @@
-// mpc.cuh — the step between two control steps of the receding-horizon controller (mbd_mpc_advance in include/mbd_b200.h).
+// mpc.cuh — the step between two control steps of the receding-horizon controller (mbd_mpc_advance and mbd_mpc_pi_advance in
+// include/mbd_b200.h).
 // k_mpc_advance: one CTA per problem, so every per-problem word has exactly one writer and no atomic is needed.  The control
 // counter c = mpc_ctl[b] is read by every thread before thread 0 advances it.
+// sigma_log == nullptr (model-based diffusion: the sigmas are the schedule's and stay): sigma_warm is not read.  Otherwise (the
+// path-integral baselines, whose update may rewrite sigma) ACT also logs params[b][0].sigma and resets rows 0 .. Nwarm to sigma_warm.
 #pragma once
 
 namespace mbd {
 
 constexpr int kMpcThreads = 256;
 
-__global__ void __launch_bounds__(kMpcThreads) k_mpc_advance(mbd_mpc_plan p, int mode) {
+__global__ void __launch_bounds__(kMpcThreads) k_mpc_advance(mbd_mpc_plan p, int mode, float sigma_warm, float* sigma_log) {
   extern __shared__ float mpc_sm[];   // [H * nu]: the plan P_c (ACT)
   const int b = blockIdx.x;
   const int tid = threadIdx.x;
@@ -40,17 +43,26 @@ __global__ void __launch_bounds__(kMpcThreads) k_mpc_advance(mbd_mpc_plan p, int
     // shift(P_c) -> Ybars[b][Nwarm]: row h takes row h + 1, the last row is 0 (the cold start's prior mean)
     float* W = Y + (size_t)nw * HNu;
     for (int k = tid; k < HNu; k += blockDim.x) W[k] = k + nu < HNu ? mpc_sm[k + nu] : 0.0f;
-    // the keys of control step c + 1 -> params[b][1 .. Nwarm].key; sigma and the coefficients stay those of the one schedule
+    // the keys of control step c + 1 -> params[b][1 .. Nwarm].key; the coefficients stay those of the one schedule, and so does
+    // sigma unless there is a sigma log: then rows 1 .. Nwarm restart from sigma_warm
     const uint32_t* kr = p.keys_dev + ((size_t)b * p.Nstep + c + 1) * nw * 2;
     mbd_step_params* sp = p.params_dev + (size_t)b * nd;
     for (int j = tid; j < nw; j += blockDim.x) {
       sp[j + 1].key[0] = kr[2 * j];
       sp[j + 1].key[1] = kr[2 * j + 1];
+      if (sigma_log) sp[j + 1].sigma = sigma_warm;
     }
   }
   __syncthreads();   // every thread has read c
   if (tid == 0) {
     p.rew_hist_log_dev[(size_t)b * p.Nstep + c] = p.rew_hist_dev[(size_t)b * nd + 1];   // rews.mean() of diffusion step 1
+    if (sigma_log) {
+      // the sigma control step c ended with: CMA-ES's last update wrote it to row 0.  MPPI and CEM never write sigma, so row 0
+      // takes sigma_warm too and their log reads the sigma they sampled with (1 at c = 0, then sigma_warm)
+      mbd_step_params* sp = p.params_dev + (size_t)b * nd;
+      sigma_log[(size_t)b * p.Nstep + c] = sp[0].sigma;
+      if (more) sp[0].sigma = sigma_warm;
+    }
     if (more) p.ctl_dev[b].i = nw;   // after the last control step the counter stays at 0, where the solve left it
     p.mpc_ctl_dev[b] = c + 1;
   }

@@ -306,6 +306,12 @@ def mpc_advance(plan: "_lib.MpcPlan", mode: int):
     check(_lib.lib().mbd_mpc_advance(ctypes.byref(plan), int(mode), _stream()), "mbd_mpc_advance")
 
 
+def mpc_pi_advance(plan: "_lib.MpcPiPlan", mode: int):
+    """mpc_advance for a controller that plans with a path-integral baseline (mbd_mpc_pi_advance): ACT also logs the sigma the
+    control step ended with and resets the next control step's sigma rows to plan.sigma_warm"""
+    check(_lib.lib().mbd_mpc_pi_advance(ctypes.byref(plan), int(mode), _stream()), "mbd_mpc_pi_advance")
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

@@ -99,6 +99,7 @@ class MpcResult:
     rewards: np.ndarray     # [B, Nstep] r_c
     states: np.ndarray      # [B, Nstep + 1, S] s_0 ... s_Nstep (the vector env's layout)
     rew_hist: np.ndarray    # [B, Nstep] rews.mean() of every control step's last diffusion step
+    sigmas: Optional[np.ndarray] = None   # [B, Nstep] the sampling sigma every control step ended with (pi_mpc only)
 
     @property
     def reward(self) -> np.ndarray:
@@ -109,21 +110,24 @@ class MpcResult:
 class Controller:
     """B closed loops of one env and shape.  `run()` replays the captured control step; `run_host_driven()` runs the same
     arithmetic with the host in the loop (eager steps, a device->host synchronisation and a host `env.step` per control step), the
-    baseline the graph-replayed loop is measured and tested against.  Each instance runs once."""
+    baseline the graph-replayed loop is measured and tested against.  Each instance runs once.
+
+    The planner is model-based diffusion.  `pi_mpc.Controller` plans with the path-integral baselines instead by overriding what
+    differs: `steps_field`, `_make_engine`, `_make_plan`, `_advance` and the two sigma hooks."""
+
+    steps_field = "Ndiffuse"   # the Args field holding the steps of the cold solve
 
     def __init__(self, env, args_list, host: bool = False):
         a0 = args_list[0]
         self.env, self.args, self.host = env, args_list, bool(host)
-        self.B, self.Nd, self.Nwarm, self.Nstep = len(args_list), a0.Ndiffuse, a0.Nwarm, a0.Nstep
+        self.B, self.Nd, self.Nwarm, self.Nstep = len(args_list), getattr(a0, self.steps_field), a0.Nwarm, a0.Nstep
         self.H, self.Nu = a0.Hsample, env.action_size
         self.device = d = torch.device("cuda", torch.cuda.current_device())
-        self.host_states, colds, warms, scheds = [], [], [], []
+        self.host_states, colds, warms = [], [], []
         for a in args_list:
-            rng_reset, cold, warm = mpc_keys(a.seed, a.Ndiffuse, a.Nwarm, a.Nstep)
+            rng_reset, cold, warm = mpc_keys(a.seed, self.Nd, a.Nwarm, a.Nstep)
             self.host_states.append(env.reset(rng_reset))   # NOTE: rng_reset as in run_diffusion
-            _, alphas, alphas_bar, sigmas = make_schedule(a.beta0, a.betaT, a.Ndiffuse)
-            print(f"init sigma = {sigmas[-1]:.2e}")
-            colds.append(cold), warms.append(warm), scheds.append((sigmas, alphas, alphas_bar))
+            colds.append(cold), warms.append(warm)
         s0 = torch.stack([env_tensors(env, s, False, d)[2].reshape(-1) for s in self.host_states]).contiguous()
         self.S = s0.shape[1]
         self.venv = None
@@ -136,10 +140,8 @@ class Controller:
                 raise ValueError(f"the vector env's state has {self.venv.state.shape[1]} words, the planner's {self.S}")
             self.venv.set_state(s0)
             state_buffer = self.venv.state
-        self.engine = e = BatchedDiffusionEngine(env, a0.Nsample, a0.Hsample, [a.temp_sample for a in args_list], False,
-                                                 self.host_states, a0.Ndiffuse, device=d, state_buffer=state_buffer)
-        e.load_schedule(colds, [s[0] for s in scheds], [s[1] for s in scheds], [s[2] for s in scheds])
-        e.set_step(self.Nd - 1)
+        self.engine = self._make_engine(colds, state_buffer)
+        self.engine.set_step(self.Nd - 1)
         self.warm_keys = np.stack(warms)                                   # [B, Nstep, Nwarm, 2] uint32
         f = dict(device=d, dtype=torch.float32)
         self.keys = torch.as_tensor(self.warm_keys.view(np.int32), device=d).contiguous()
@@ -151,6 +153,18 @@ class Controller:
         self.graph = None
         self.warm_seconds = 0.0    # wall time of control steps 1 ... Nstep - 1 of the last run (synchronised at both ends)
         self.plan = self._make_plan() if not self.host else None
+
+    def _make_engine(self, colds, state_buffer):
+        """the planner of all B loops, reading its initial states from state_buffer, with the cold solve's schedule loaded"""
+        a0, scheds = self.args[0], []
+        for a in self.args:
+            _, alphas, alphas_bar, sigmas = make_schedule(a.beta0, a.betaT, a.Ndiffuse)
+            print(f"init sigma = {sigmas[-1]:.2e}")
+            scheds.append((sigmas, alphas, alphas_bar))
+        e = BatchedDiffusionEngine(self.env, a0.Nsample, a0.Hsample, [a.temp_sample for a in self.args], False, self.host_states,
+                                   a0.Ndiffuse, device=self.device, state_buffer=state_buffer)
+        e.load_schedule(colds, [s[0] for s in scheds], [s[1] for s in scheds], [s[2] for s in scheds])
+        return e
 
     def _make_plan(self) -> "_lib.MpcPlan":
         p = _lib.MpcPlan()
@@ -166,9 +180,19 @@ class Controller:
     # ---- the device loop --------------------------------------------------------------------------------------------------
     def _execute(self):
         """ACT, the env step and RECORD: a_c into the plant, s_{c+1} and r_c into the logs, the next control step re-armed"""
-        ops.mpc_advance(self.plan, _lib.MPC_ACT)
+        self._advance(_lib.MPC_ACT)
         ops.vec_step(self.venv.plan)
-        ops.mpc_advance(self.plan, _lib.MPC_RECORD)
+        self._advance(_lib.MPC_RECORD)
+
+    def _advance(self, mode: int):
+        ops.mpc_advance(self.plan, mode)
+
+    def _sigma_log(self) -> Optional[np.ndarray]:
+        """MpcResult.sigmas: model-based diffusion's sigmas are its schedule's, so it logs none"""
+        return None
+
+    def _host_sigma(self, c: int, more: bool):
+        """the host-driven loop's share of what ACT does to the sampling sigmas at control step c (nothing for this planner)"""
 
     def _warm_step(self):
         for _ in range(self.Nwarm):
@@ -218,7 +242,7 @@ class Controller:
 
     def result(self) -> MpcResult:
         n = lambda t: t.detach().cpu().numpy()   # noqa: E731
-        return MpcResult(n(self.actions), n(self.rewards), n(self.states), n(self.rew_hist))
+        return MpcResult(n(self.actions), n(self.rewards), n(self.states), n(self.rew_hist), self._sigma_log())
 
     # ---- the host-driven loop ---------------------------------------------------------------------------------------------
     def run_host_driven(self) -> MpcResult:
@@ -248,6 +272,7 @@ class Controller:
                     sts[b, c + 1] = host_raw(env, st[b])
                     rews[b, c] = np.float32(st[b].reward)
                 acts[:, c] = a
+                self._host_sigma(c, c + 1 < self.Nstep)
                 if c + 1 < self.Nstep:
                     e.state_init.copy_(torch.as_tensor(sts[:, c + 1], device=self.device))
                     e.Ybars[:, nw].copy_(shift(P).reshape(B, -1))
@@ -256,7 +281,7 @@ class Controller:
             torch.cuda.synchronize()
             self.warm_seconds = time.perf_counter() - t0 if self.Nstep > 1 else 0.0
             e.check_exchange()
-        return MpcResult(acts, rews, sts, rh)
+        return MpcResult(acts, rews, sts, rh, self._sigma_log())
 
 
 def host_raw(env, state) -> np.ndarray:
@@ -297,8 +322,8 @@ def run_mpc(args: Args, log_every: int = 10, return_result: bool = False):
     return (rew, res) if return_result else rew
 
 
-def _render(env, states: np.ndarray, path: str):
-    """the executed states s_0 ... s_Nstep: the Brax-visualizer page (positional envs, pushT) or car2d's plot"""
+def _render(env, states: np.ndarray, path: str, name: str = "mpc_rollout"):
+    """the executed states s_0 ... s_Nstep: the Brax-visualizer page {name}.html (positional envs, pushT) or car2d's plot {name}.png"""
     if env.kind == "car2d":
         try:
             import matplotlib
@@ -309,7 +334,7 @@ def _render(env, states: np.ndarray, path: str):
         fig, ax = plt.subplots(1, 1, figsize=(3, 3))
         env.render(ax, states)
         ax.legend()
-        plt.savefig(f"{path}/mpc_rollout.png")
+        plt.savefig(f"{path}/{name}.png")
         plt.close(fig)
         return
     from ..io import brax_json
@@ -317,7 +342,7 @@ def _render(env, states: np.ndarray, path: str):
         rollout = [env._make_pipeline_state(s.reshape(-1, 13)) for s in states]
     else:
         rollout = [env.pipeline_init(s[:8], s[8:]) for s in states]
-    with open(f"{path}/mpc_rollout.html", "w") as f:
+    with open(f"{path}/{name}.html", "w") as f:
         f.write(brax_json.render(env.sys, rollout, env.dt))
 
 
