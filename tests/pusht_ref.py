@@ -53,7 +53,8 @@ Part 2, the solver.
   derivation of the remaining distance survives the dependent rows of a contact (the iteration matrix on the 3 rows of a
   contact has a unit eigenvalue along the null space of J^T), so the truncation radius is a STATED CONSTANT: C_TRUNC * TOL *
   |F|_inf on every component of the force F = J^T x, C_TRUNC = 4 x the largest |production - fixed point| / (TOL |F|_inf
-  pushed through the integration) measured over all families (tests/pusht_families.py).
+  pushed through the integration) measured over all families (tests/pusht_families.py); along the substep chains of
+  tests/pusht_chain.py the largest is 1.76 x less than C_TRUNC (TRUNC_MEASURED below).
 The force radius is |J_:k|_2 e + sum_i rJ_ik (|x_i| + e) + gamma_{m+1} (|qf_k| + sum_i |J_ik x_i|); the integration
 charges the solve of (M + dt D) its Gaussian-elimination backward error gamma_12 |M| (the elimination of the two slides
 first, the kernel's closed form, has |L||U| = |M|) plus the radii of its entries, then one rounding per `qd + dt qdd`.
@@ -82,9 +83,14 @@ PI_F = float(np.float32(np.pi))
 PATHS = ("none", "fast4-box0", "fast4-box1", "solve4", "solve8", "solve12")
 # production-mode truncation: C_TRUNC * TOL * |J^T x|_inf on every force component, a measured constant (module docstring):
 # 4 x the largest ratio measured over every family at mu = 1 and mu = 0 (2833, mu = 0 limits plus one contact;
-# tests/test_pusht_ref_cpu.py::test_truncation_constant pins it)
-TRUNC_MEASURED = 2900.0
-C_TRUNC = 4.0 * TRUNC_MEASURED
+# tests/test_pusht_ref_cpu.py::test_truncation_constant pins it).  Over the families and the substep chains of
+# tests/pusht_chain.py together the largest ratio is 6577 (tests/test_pusht_horizon_ref_cpu.py pins it): mu = 0, the pusher
+# pressed into the re-entrant corner by the scripted push from the `speeds` start, both contacts active (solve8), where
+# Gauss-Seidel contracts so slowly that a sweep moving the force by TOL |F| still leaves it 6.6e-3 |F| from the fixed point.
+# C_TRUNC is kept: 1.76 x that figure
+TRUNC_FAMILIES = 2900.0
+TRUNC_MEASURED = 6600.0
+C_TRUNC = 4.0 * TRUNC_FAMILIES
 
 
 def _f(P, name, k=0):
@@ -515,13 +521,14 @@ def _one_config(P, st, u, geo):
         value[:, k], radius[:, k] = p1.v, p1.r
         trunc[:, 8 + k] = tq[:, k] * dt * (1 + 4 * U)
         trunc[:, k] = trunc[:, 8 + k] * dt * (1 + 4 * U)
-    out.update(value=value, radius=radius, trunc=trunc, x3=x3, F=F)
+    out.update(value=value, radius=radius, trunc=trunc, x3=x3, F=F, impulse=dt * (F @ Minti.T))
     return out
 
 
 def step(P, st, u):
     """one physics step of pushT for one fp32 state [16] and fp32 controls [n, 2] (clipped here like the kernel) ->
-    dict(value [n, 16], radius_fixed, trunc_unit [n, 16], undecided [n], path, nrows, straddle, kkt, merge_gap)"""
+    dict(value [n, 16], radius_fixed, trunc_unit [n, 16], undecided [n], path, nrows, straddle, kkt, merge_gap, configs: per
+    enumerated gate outcome, among others the velocity change of the constraint impulse, impulse [n, 5] = dt (M + dt D)^-1 J^T x)"""
     P = np.asarray(P, dtype=np.float32).astype(np.float64)
     st = np.asarray(st, dtype=np.float32).astype(np.float64)
     u = np.clip(np.asarray(u, dtype=np.float32).astype(np.float64), -1.0, 1.0)

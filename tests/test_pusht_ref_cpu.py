@@ -93,7 +93,9 @@ def test_oracle_within_the_bound(cases, mode):
 
 def test_truncation_constant(cases):
     """the production-mode truncation radius is the stated constant C_TRUNC = 4 x the largest ratio |production - fixed
-    point| / unit truncation radius over every family; pin the measurement it was taken from"""
+    point| / unit truncation radius over every family; pin the measurement it was taken from.  The substep chains reach
+    larger ratios (tests/test_pusht_horizon_ref_cpu.py::test_truncation_constant_along_the_chains pins TRUNC_MEASURED, the
+    largest over both), still below C_TRUNC"""
     worst = 0.0
     for (mu, fam), launches in cases.items():
         for P, st, u, ref in launches:
@@ -102,7 +104,8 @@ def test_truncation_constant(cases):
                 q = np.where(d == 0, 0.0, d / ref["trunc"])
             worst = max(worst, float(q[~ref["undecided"]].max(initial=0.0)))
     print("largest truncation ratio", worst)
-    assert 0.5 * X.TRUNC_MEASURED <= worst <= X.TRUNC_MEASURED and X.C_TRUNC == 4.0 * X.TRUNC_MEASURED
+    assert 0.5 * X.TRUNC_FAMILIES <= worst <= X.TRUNC_FAMILIES and X.C_TRUNC == 4.0 * X.TRUNC_FAMILIES
+    assert X.TRUNC_FAMILIES <= X.TRUNC_MEASURED < X.C_TRUNC
 
 
 def test_the_bound_is_not_vacuous(cases):
