@@ -26,8 +26,9 @@ The step (car2d.py:77-86):
 
 Branch gate.  Obstacle k's margin dist_k - r carries dist_k's radius.  The car surely collides where some margin is below
 minus its radius.  Where no obstacle surely collides and some margin is within its radius, the outcome is undecided: the
-result is the interval hull of q and q_new, and the sample is marked `undecided` (the tests exclude it and bound how many
-there are) when the two outcomes differ by more than JUMP radii in some word, the rule of tests/xpbd_ref.py.
+result is the interval hull of q and q_new, and the sample is marked `undecided` when the two outcomes differ by more than
+JUMP radii in some word, the rule of tests/xpbd_ref.py.  An undecided step is held to one of the two outcomes
+(`check_rollout_branches`): it equals the frozen q bit for bit (q is an exact input) or lies within K radii of q_new.
 
 `reward` (car2d.py:88-93) and `logpd` (car2d.py:95-102) evaluate the kernel's per-step reward and demo log-density on given
 fp32 states.  For a horizon H longer than the reference path (href rows), step t >= href is compared with the last row,
@@ -83,7 +84,8 @@ def rk4(P, states, actions):
 
 def step(P, states, actions):
     """one env step of states [n, 3] under actions [n, 2] -> dict(value [n, 3], radius [n, 3], undecided [n], collide [n]
-    (surely collides), straddle [n] (some margin within its radius, no sure collision))"""
+    (surely collides), straddle [n] (some margin within its radius, no sure collision), new_value / new_radius [n, 3]
+    (the outcome without collision, q_new))"""
     T = table(P)
     s = _f64(states)
     q = tuple(R(s[:, i].copy()) for i in range(3))
@@ -105,7 +107,8 @@ def step(P, states, actions):
         out[i] = R(np.where(straddle, 0.5 * (q[i].v + qn[i].v), out[i].v),
                    np.where(straddle, 0.5 * gap + np.maximum(q[i].r, qn[i].r), out[i].r))
     return dict(value=np.stack([c.v for c in out], -1), radius=np.stack([c.r for c in out], -1),
-                undecided=straddle & jump, collide=sure, straddle=straddle)
+                undecided=straddle & jump, collide=sure, straddle=straddle,
+                new_value=np.stack([c.v for c in qn], -1), new_radius=np.stack([c.r for c in qn], -1))
 
 
 def clamp_hi(x, hi):
@@ -169,3 +172,37 @@ def check_rollout(P, x0, Y, out, xref=None):
         lp = logpd(traj, xref)
         res["logpd"] = ratio(out["logpd"], lp.v, lp.r)
     return res
+
+
+def held_steps(prev, got, ref):
+    """the undecided steps held to one outcome: the frozen state q (an exact input, so taking the collision branch means
+    equal bit for bit) or within K radii of q_new.  prev [m, 3] the state before, got [m, 3] the state after, ref = step(P,
+    prev, Y) -> (best [u], second [u]) over the u undecided steps: the ratio to the nearer outcome (0 for q itself) and to
+    the other one, both in radii of q_new"""
+    und = ref["undecided"]
+    old = np.asarray(prev, np.float32)[und]
+    g = np.asarray(got, np.float32)[und]
+    frozen = np.array([np.array_equal(a.view(np.uint32), b.view(np.uint32)) for a, b in zip(g, old)], dtype=bool)
+    to_new = np.zeros(len(g))
+    for j in range(len(g)):
+        to_new[j] = ratio(g[j], ref["new_value"][und][j], ref["new_radius"][und][j])
+    to_old = np.zeros(len(g))
+    for j in range(len(g)):
+        to_old[j] = ratio(g[j], old[j].astype(np.float64), ref["new_radius"][und][j])
+    best = np.where(frozen, 0.0, to_new)
+    second = np.where(frozen, to_new, to_old)
+    return best, second
+
+
+def check_rollout_branches(P, x0, Y, out):
+    """check_rollout's teacher-forced steps with every undecided step held to one branch outcome (held_steps) -> dict(held,
+    undecided, unchecked (always 0: both outcomes are known), ratio (largest held), second [per held step])"""
+    Y = np.asarray(Y, dtype=np.float32)
+    n, H, _ = Y.shape
+    traj = np.asarray(out["traj"], dtype=np.float32)
+    start = np.broadcast_to(np.asarray(x0, dtype=np.float32).reshape(-1, 1, 3), (n, 1, 3))
+    prev = np.concatenate([start, traj[:, :-1]], 1).reshape(-1, 3)
+    ref = step(P, prev, Y.reshape(-1, 2))
+    best, second = held_steps(prev, traj.reshape(-1, 3), ref)
+    return dict(held=len(best), undecided=int(ref["undecided"].sum()), unchecked=0, ratio=float(best.max(initial=0.0)),
+                second=second, best=best)

@@ -136,6 +136,28 @@ class StepMemo:
 
     def __init__(self):
         self.rows = {}
+        self.branch_rows = {}
+
+    def branches(self, blob, states, actions):
+        """the forced-branch outcomes (xpbd_ref.branch_outcomes) of every undecided row -> [(row index, (value [A, L, 13],
+        radius, valid [A, L], whole, still, nsites))], memoised like the step itself"""
+        states = np.ascontiguousarray(states, dtype=np.float32)
+        actions = np.ascontiguousarray(actions, dtype=np.float32)
+        _, _, und = self(blob, states, actions)
+        tag = np.ascontiguousarray(blob, dtype=np.uint32).tobytes()
+        keys = {i: (tag, states[i].tobytes(), actions[i].tobytes()) for i in np.flatnonzero(und)}
+        todo = {}
+        for i, k in keys.items():
+            if k not in self.branch_rows:
+                todo.setdefault(k, i)
+        if todo:
+            idx = list(todo.values())
+            ref = X.positional_step(blob, states[idx], actions[idx])
+            br = X.branch_outcomes(blob, states[idx], actions[idx], ref)
+            for j, r in enumerate(br["rows"]):
+                self.branch_rows[keys[idx[r]]] = (br["value"][j], br["radius"][j], br["valid"][j], bool(br["whole"][j]),
+                                                  bool(br["still"][j]), int(br["nsites"][j]))
+        return [(i, self.branch_rows[k]) for i, k in keys.items()]
 
     def __call__(self, blob, states, actions):
         """states [n, L, 13], actions [n, nu] -> (value [n, L, 13], radius [n, L, 13], undecided [n])"""
@@ -162,6 +184,26 @@ def step_ratio(memo, blob, prev, u, got):
     value, radius, und = memo(blob, prev, u)
     ok = np.broadcast_to(~und[:, None, None], value.shape)
     return ratio(got, value, radius, ok), int(und.sum())
+
+
+def step_ratios(memo, blob, prev, u, got):
+    """step_ratio with the undecided samples held to their forced branches (xpbd_ref.held_ratios) -> (largest ratio over the
+    decided samples, largest best-assignment ratio over the undecided ones, count still unchecked, dict(undecided, held
+    [ratio per held sample], second [distance to the second-best assignment per held sample]))"""
+    value, radius, und = memo(blob, prev, u)
+    ok = np.broadcast_to(~und[:, None, None], value.shape)
+    dec = ratio(got, value, radius, ok)
+    held, second, unchecked = [], [], 0
+    got = np.asarray(got)
+    for i, (v, r, valid, whole, still, _) in memo.branches(blob, prev, u):
+        if still:
+            unchecked += 1
+            continue
+        br = dict(rows=[i], value=v[None], radius=r[None], valid=valid[None], whole=[whole])
+        b, s = X.held_ratios(got[i][None], br)
+        held.append(float(b[0]))
+        second.append(float(s[0]))
+    return dec, max(held, default=0.0), unchecked, dict(undecided=int(und.sum()), held=held, second=second)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -587,3 +587,21 @@ def mean_return(rewss):
     H = r.shape[1]
     tot = fsum([R(r[:, t]) for t in range(H)])
     return tot / float(H)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# undecided samples: held to one enumerated configuration
+# ---------------------------------------------------------------------------------------------------------------------
+def held_ratios(got, ref, mode):
+    """got [n, 16] against every enumerated gate configuration of ref = step(...) in a solver mode -> (best [u], second [u])
+    over the u undecided samples: the largest ratio to the nearest configuration, and to the next-nearest (inf with one)"""
+    und = ref["undecided"]
+    g = np.asarray(got, dtype=np.float64)[und]
+    per = []
+    for cfg in ref["configs"]:
+        d = np.abs(g - cfg["value"][und])
+        with np.errstate(divide="ignore", invalid="ignore"):
+            q = np.where(d == 0, 0.0, d / radius(cfg, mode)[und])
+        per.append(np.where(np.isfinite(d), q, np.inf).max(1))
+    per = np.sort(np.stack(per), axis=0)
+    return per[0], (per[1] if len(per) > 1 else np.full(len(g), np.inf))

@@ -25,11 +25,14 @@ Error model, u = 2^-24:
   plus 8 roundings for the operations folded away.
 
 Branches: where the margin of a discontinuous predicate is within its radius, the result is the interval hull of both
-outcomes; when the two outcomes differ by more than JUMP times the radius, the sample is also marked `undecided` and the
-tests exclude it and bound how many there may be.  Predicates: the static-friction test |dl_t| < mu |dl|, the sinking
-gate v_n_old <= 0, the contact test dist < 0 (the normal velocity impulse does not vanish with dl), the `dq.w >= 0` sign of
-project_xd, and the atan2 branch cut at +-pi where the angle feeds a spring or a finite limit.  Clamps, min and |.| are
-Lipschitz and need no gate.
+outcomes; when the two outcomes differ by more than JUMP times the radius, that predicate instance is a gated SITE and the
+sample is marked `undecided`.  Predicates: the static-friction test |dl_t| < mu |dl|, the sinking gate v_n_old <= 0, the
+contact test dist < 0 (the normal velocity impulse does not vanish with dl), the `dq.w >= 0` sign of project_xd, and the
+atan2 branch cut at +-pi where the angle feeds a spring or a finite limit.  Clamps, min and |.| are Lipschitz and need no
+gate.  A fp32 evaluation whose margin is within the radius may take either outcome, and downstream of it computes that
+outcome's formula, so an undecided sample is held to the evaluations with its sites FORCED (`positional_step(force=)`,
+`branch_outcomes`): it must lie within K radii of one consistent assignment of outcomes.  The contact test is one variable
+per (link, contact slot), read by both the position stage and the velocity stage.
 
 `reward_*` evaluate the per-step rewards the kernels compute (upstream humanoidrun.py:46-51, humanoidstandup.py:50-56,
 hopper.py:57-65, walker2d.py:56-61, cartpole.py:44, humanoidtrack.py:87-106, ant [brax-recalled]) on a given fp32 state,
@@ -283,16 +286,22 @@ def norm_bound(v):
     return np.sqrt(sum(c.v * c.v for c in v)) + sum(c.r for c in v)
 
 
-def dead_zone(a, cut, lo, hi, gate):
+def other_reading(a):
+    """the angle on the other side of the atan2 branch cut: a - 2 pi sign(a), with a's radius"""
+    return R(a.v - 2 * np.pi * np.sign(a.v), a.r)
+
+
+def dead_zone(a, cut, lo, hi, decide):
     """a - clip(a, lo, hi): exactly 0 where a is inside the band by more than its radius.  At an atan2 branch cut both
-    +-pi readings must give 0, otherwise the sample is undecided."""
-    e = _round(a.v - np.clip(a.v, lo, hi), a.r)
-    inside = (a.v - a.r > lo) & (a.v + a.r < hi)
-    e = R(np.where(inside, 0.0, e.v), np.where(inside, 0.0, e.r))
-    alt = a.v - 2 * np.pi * np.sign(a.v)
-    alt_inside = (alt - a.r > lo) & (alt + a.r < hi)
-    gate("atan2 cut (limit)", cut & ~(inside & alt_inside))
-    return e
+    +-pi readings must give 0, otherwise the reading is a gated site: decide(within, natural) picks it."""
+    def excess(x):
+        e = _round(x.v - np.clip(x.v, lo, hi), x.r)
+        inside = (x.v - x.r > lo) & (x.v + x.r < hi)
+        return R(np.where(inside, 0.0, e.v), np.where(inside, 0.0, e.r)), inside
+    e, inside = excess(a)
+    e_alt, alt_inside = excess(other_reading(a))
+    keep = decide(cut & ~(inside & alt_inside), np.ones_like(cut, dtype=bool))
+    return where(keep, e, e_alt)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -389,20 +398,64 @@ def _slide_axis(k, parity, a_p, shape):
 # ---------------------------------------------------------------------------------------------------------------------
 # one substep
 # ---------------------------------------------------------------------------------------------------------------------
-def positional_step(blob, states, actions):
+SITES = ("static friction", "sinking gate", "dist < 0", "dq.w >= 0", "atan2 cut (spring)", "atan2 cut (limit)")
+
+
+def positional_step(blob, states, actions, force=None, strict=True):
     """states [n, L, 13] fp32, actions [n, nu] fp32 -> dict(value [n, L, 13], radius [n, L, 13], undecided [n],
-    reasons {predicate: [n] mask})"""
+    reasons {predicate: [n] mask}, sites {site: [n, L] mask})
+
+    A site is one predicate instance: (predicate, contact slot) for the three contact predicates, (predicate, dof) for the
+    two atan2 cuts, (predicate,) for dq.w; its masks are per (sample, link).  `sites` holds the gated instances that made
+    a sample undecided, and `outcomes` the outcome every instance took.  `force` maps a site to an int8 array [n, L]: -1
+    leaves the instance free, 0 / 1 take the outcome False / True (for a cut, True is the angle atan2 computes and False
+    the other reading a - 2 pi sign(a)).  A forced outcome replaces the hull where the instance is gated; where its margin
+    is within its radius but the outcomes are closer than JUMP radii, the hull stays (the contact test still takes the
+    forced outcome in the position stage: it covers both).  Forcing an instance whose margin is outside its radius to the
+    outcome float64 does not take is an error (with strict=False it is recorded in `infeasible` [n, L] and the decided
+    outcome is taken: another forced site decided this one); forcing it to that outcome changes nothing."""
     m = Model(blob)
     states = np.asarray(states, dtype=np.float32).astype(np.float64)
     actions = np.asarray(actions, dtype=np.float32).astype(np.float64)
     n, L = states.shape[0], m.L
     shape = (n, L)
     reasons = {}
+    sites = {}
+    outcomes = {}
+    infeasible = np.zeros(shape, dtype=bool)
+    force = {} if force is None else force
 
-    def gate(name, mask):
-        """marks the samples where a discontinuous predicate is within its radius"""
-        m_ = np.broadcast_to(mask, shape).any(axis=-1)
-        reasons[name] = reasons.get(name, np.zeros(n, dtype=bool)) | m_
+    def gate(name, mask, key=None):
+        """marks the samples where a discontinuous predicate is within its radius and its outcomes jump"""
+        mask = np.broadcast_to(mask, shape)
+        reasons[name] = reasons.get(name, np.zeros(n, dtype=bool)) | mask.any(axis=-1)
+        if key is not None and mask.any():
+            sites[key] = sites.get(key, np.zeros(shape, dtype=bool)) | mask
+
+    def forced(key, within, natural):
+        """(outcome, forced mask) of a predicate instance: float64's own outcome `natural` unless `force` takes one where
+        the margin is `within` its radius"""
+        within = np.broadcast_to(within, shape)
+        natural = np.broadcast_to(natural, shape)
+        f = force.get(key)
+        if f is None:
+            outcomes[key] = natural
+            return natural, np.zeros(shape, dtype=bool)
+        f = np.broadcast_to(np.asarray(f, dtype=np.int8), shape)
+        bad = (f >= 0) & ~within & ((f == 1) != natural)
+        infeasible[...] |= bad
+        if bad.any() and strict:
+            raise ValueError(f"{key} forced against a decided outcome at {np.argwhere(bad)[:4].tolist()}")
+        fm = (f >= 0) & within
+        out = np.where(fm, f == 1, natural)
+        outcomes[key] = out
+        return out, fm
+
+    def decide(key, gated, natural):
+        """the outcome of a predicate instance gated on `gated` (within its radius, outcomes over JUMP radii apart)"""
+        out, fm = forced(key, gated, natural)
+        gate(key[0], gated & ~fm, key)
+        return out
 
     def col(k):
         return R(states[:, :, k].copy())
@@ -449,8 +502,8 @@ def positional_step(blob, states, actions):
         ak = _slide_axis(k, parity, a_p, shape)
         f = fsum([tau, -(dot(d_s, ak) * stiff), -(dot(va_s, ak) * damp)])
         vel = dot(ea["ax"][k], jd)
-        t = fsum([tau, -(ea["ang"][k] * stiff), -(vel * damp)])
-        gate("atan2 cut (spring)", ea["cut"][k] & exists & ~is_slide & (stiff != 0))
+        keep = decide(("atan2 cut (spring)", k), ea["cut"][k] & exists & ~is_slide & (stiff != 0), np.ones(shape, dtype=bool))
+        t = fsum([tau, -(where(keep, ea["ang"][k], other_reading(ea["ang"][k])) * stiff), -(vel * damp)])
         hinge = exists & ~is_slide
         for i in range(3):
             tq_terms[i].append(where(hinge, ea["ax"][k][i] * t, 0.0))
@@ -506,7 +559,8 @@ def positional_step(blob, states, actions):
     for k in range(B.MAXDOF):
         is_slide = ((smask >> k) & 1) == 1
         used = jointed & ~is_slide & ((k == 0) | (ndof > 1))      # a 1-dof joint aligns its axis instead of using angles 1, 2
-        ek = dead_zone(ea["ang"][k], ea["cut"][k] & used, dof(k, B.D_LO), dof(k, B.D_HI), gate)
+        ek = dead_zone(ea["ang"][k], ea["cut"][k] & used, dof(k, B.D_LO), dof(k, B.D_HI),
+                       lambda within, nat, k=k: decide(("atan2 cut (limit)", k), within, nat))
         err.append(where(is_slide, ea["ang"][k], ek))
     one = ndof == 1
     dqj3 = tuple(fsum([ea["ax"][k][i] * err[k] for k in range(3)]) for i in range(3))
@@ -541,8 +595,8 @@ def positional_step(blob, states, actions):
         rad, mu = m.lf(base + 3), m.lf(base + 4)
         centre = vadd(p, rotate(S, q))
         dist = centre[2] - rad
-        coll = dist.v < 0
         near = active & (np.abs(dist.v) <= dist.r)
+        coll, coll_fm = forced(("dist < 0", ci), near, dist.v < 0)   # one outcome for the position and velocity stages
         cp = (centre[0], centre[1], centre[2] - fsum([rad, exact_scale(dist, 0.5)]))
         r = vsub(cp, p)
         wn = fsum([im, r[0] * r[0], r[1] * r[1]])
@@ -559,8 +613,10 @@ def positional_step(blob, states, actions):
         stat = coll & (margin.v > 0)
         Pt = tuple(extra(-x / Wt, 8) for x in dxy)
         either = active & coll & (np.abs(margin.v) <= margin.r) & (margin.r > 0)
-        gate("static friction", either & (dlt.v > JUMP * dlt.r))
-        Pt = vwhere(either, hull(Pt), vwhere(stat, Pt, (zero,) * 3))
+        stat, fm = forced(("static friction", ci), either, stat)
+        gated = either & (dlt.v > JUMP * dlt.r)
+        gate("static friction", gated & ~fm, ("static friction", ci))
+        Pt = vwhere(either & ~(fm & gated), hull(Pt), vwhere(stat, Pt, (zero,) * 3))
         Pt = (Pt[0], Pt[1], dl)
         dpl = vscale(Pt, im)
         dql = tuple(exact_scale(x, 0.5) for x in qmul(pure(cross(r, Pt)), q))
@@ -568,7 +624,7 @@ def positional_step(blob, states, actions):
             dp_acc[i].append(where(active, dpl[i], 0.0))
         for i in range(4):
             dq_acc[i].append(where(active, dql[i], 0.0))
-        contacts.append((active, cp, dl, coll, mu, near))
+        contacts.append((ci, active, cp, dl, coll, mu, near, coll_fm))
     if contacts:
         has_con = ncon > 0
         dpt = tuple(fsum(t) for t in dp_acc)
@@ -579,8 +635,8 @@ def positional_step(blob, states, actions):
     # ---- project_xd: velocities from the positional change
     v = tuple((p[i] - p_prev[i]) * m.inv_dt for i in range(3))
     dq = qmul(q, conj(q_prev))
-    gate("dq.w >= 0", (np.abs(dq[0].v) <= dq[0].r) & (dq[0].r > 0))
-    sgn = np.where(dq[0].v >= 0, m.two_inv_dt, -m.two_inv_dt)
+    pos = decide(("dq.w >= 0",), (np.abs(dq[0].v) <= dq[0].r) & (dq[0].r > 0), dq[0].v >= 0)
+    sgn = np.where(pos, m.two_inv_dt, -m.two_inv_dt)
     w = tuple(dq[i] * sgn for i in (1, 2, 3))
 
     # ---- velocity solve: dynamic friction, restitution, normal velocity of approaching contacts
@@ -588,7 +644,7 @@ def positional_step(blob, states, actions):
         dv_acc = [[], [], []]
         dw_acc = [[], [], []]
         v0, w0 = v, w
-        for active, cp, dl, coll, mu, near in contacts:
+        for ci, active, cp, dl, coll, mu, near, coll_fm in contacts:
             r = vsub(cp, p)
             rel = vadd(v0, cross(w0, r))
             vn = rel[2]
@@ -609,11 +665,12 @@ def positional_step(blob, states, actions):
             rest = rmin(-(vn_old * m.elasticity), 0.0)
             wn = fsum([im, r[0] * r[0], r[1] * r[1]])
             prz = fsum([-vn, rest]) * (1.0 / (wn + EPS))
-            gate("sinking gate", active & coll & (np.abs(vn_old.v) <= vn_old.r) & (vn_old.r > 0))
-            Pz = where(vn_old.v <= 0, prz, 0.0)
+            sink = decide(("sinking gate", ci), active & coll & (np.abs(vn_old.v) <= vn_old.r) & (vn_old.r > 0), vn_old.v <= 0)
+            Pz = where(sink, prz, 0.0)
             Pv = (Pd[0], Pd[1], Pz)
-            gate("dist < 0", near & (np.abs(Pz.v) > JUMP * Pz.r))
-            Pv = vwhere(near, tuple(hull(x) for x in Pv), vwhere(coll, Pv, (zero,) * 3))
+            gated = near & (np.abs(Pz.v) > JUMP * Pz.r)
+            gate("dist < 0", gated & ~coll_fm, ("dist < 0", ci))
+            Pv = vwhere(near & ~(coll_fm & gated), tuple(hull(x) for x in Pv), vwhere(coll, Pv, (zero,) * 3))
             dvl = vscale(Pv, im)
             dwl = cross(r, Pv)
             for i in range(3):
@@ -629,7 +686,111 @@ def positional_step(blob, states, actions):
     undecided = np.zeros(n, dtype=bool)
     for m_ in reasons.values():
         undecided |= m_
-    return dict(value=value, radius=radius, undecided=undecided, reasons=reasons)
+    return dict(value=value, radius=radius, undecided=undecided, reasons=reasons, sites=sites, outcomes=outcomes,
+                infeasible=infeasible)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# undecided samples: the outcomes of their sites, forced
+# ---------------------------------------------------------------------------------------------------------------------
+MAX_BITS = 10    # at most 2^10 forced evaluations per sample; a sample needing more is left unchecked
+
+
+def instances(sites, i, L):
+    """[(site, link)] of sample i, links ascending"""
+    return [(key, l) for l in range(L) for key in sorted(sites) if sites[key][i, l]]
+
+
+def branch_outcomes(blob, states, actions, ref):
+    """the undecided samples of ref = positional_step(blob, states, actions) under assignments of their sites.
+
+    After the joint solve, the contact stage, project_xd and the velocity solve act on one link at a time, so a link's 13
+    words depend only on its own contact and dq.w sites: pass a forces bit j of a to the j-th site of EVERY link, and one
+    pass gives each link its outcome under assignment a (2^(largest site count of a link) passes).  An atan2 cut couples
+    links through the acceleration update and the joint solve, so a sample with a cut site is enumerated as a whole: bit j
+    to the sample's j-th site.
+    -> dict(rows [m] sample indices, value / radius [m, A, L, 13], valid [m, A, L] (a is an assignment of link l's own sites,
+    or every a for a whole-sample enumeration), whole [m], still [m] (a forced evaluation gated a new site, or more than
+    MAX_BITS sites: unchecked), nsites [m]).  An assignment under which one forced site decides another against its forced
+    outcome (the sinking gate of a contact forced not to collide, say) is infeasible and not valid."""
+    m = Model(blob)
+    L = m.L
+    states = np.asarray(states, dtype=np.float32)
+    actions = np.asarray(actions, dtype=np.float32)
+    rows = np.flatnonzero(ref["undecided"])
+    sites = ref["sites"]
+    info = []
+    for i in rows:
+        inst = instances(sites, i, L)
+        whole = any(key[0].startswith("atan2") for key, _ in inst)
+        if whole:
+            bit = {(key, l): j for j, (key, l) in enumerate(inst)}
+            nb = len(inst)
+        else:
+            bit, cnt = {}, [0] * L
+            for key, l in inst:
+                bit[(key, l)] = cnt[l]
+                cnt[l] += 1
+            nb = max(cnt)
+        info.append((whole, bit, nb, len(inst)))
+    A = 1 << min(max([nb for _, _, nb, _ in info if nb <= MAX_BITS], default=0), MAX_BITS)
+    M = len(rows)
+    value = np.full((M, A, L, 13), np.nan)
+    radius = np.full((M, A, L, 13), np.nan)
+    valid = np.zeros((M, A, L), dtype=bool)
+    still = np.array([nb > MAX_BITS for _, _, nb, _ in info], dtype=bool)
+    for nb in sorted({nb for _, _, nb, _ in info if nb <= MAX_BITS}):
+        g = [j for j, x in enumerate(info) if x[2] == nb]
+        for a in range(1 << nb):
+            force = {}
+            for gj, j in enumerate(g):
+                for (key, l), b in info[j][1].items():
+                    f = force.setdefault(key, np.full((len(g), L), -1, dtype=np.int8))
+                    f[gj, l] = (a >> b) & 1
+            out = positional_step(blob, states[rows[g]], actions[rows[g]], force, strict=False)
+            for gj, j in enumerate(g):
+                value[j, a], radius[j, a] = out["value"][gj], out["radius"][gj]
+                still[j] |= bool(out["undecided"][gj])
+                whole, bit = info[j][0], info[j][1]
+                bad = out["infeasible"][gj]
+                if whole:
+                    valid[j, a] = not bad.any()
+                else:
+                    cnt = np.zeros(L, dtype=int)
+                    for (_, l) in bit:
+                        cnt[l] += 1
+                    valid[j, a] = (a < (1 << cnt)) & ~bad
+    return dict(rows=rows, value=value, radius=radius, valid=valid, whole=np.array([x[0] for x in info], dtype=bool),
+                still=still, nsites=np.array([x[3] for x in info], dtype=int))
+
+
+def _word_ratio(got, value, radius):
+    d = np.abs(np.asarray(got, dtype=np.float64) - value)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        q = np.where(d == 0, 0.0, d / radius)
+    return np.where(np.isfinite(d), q, np.inf)
+
+
+def held_ratios(got, br):
+    """got [m, L, 13] (the rows of `br`) -> (best [m], second [m]): the largest ratio of the sample to its best consistent
+    assignment (each link's minimum over its own assignments, or the minimum over whole-sample assignments), and the same
+    for the second-best assignment of the link (or sample) where it is closest (inf with a single assignment)"""
+    got = np.asarray(got)
+    M = len(br["rows"])
+    best, second = np.zeros(M), np.full(M, np.inf)
+    for j in range(M):
+        q = _word_ratio(got[j][None], br["value"][j], br["radius"][j]).max(-1)        # [A, L]
+        q = np.where(br["valid"][j], q, np.inf)
+        if br["whole"][j]:
+            per = np.sort(q.max(1))
+            best[j] = per[0]
+            second[j] = per[1] if len(per) > 1 else np.inf
+        else:
+            per = np.sort(q, axis=0)                                                  # [A, L]
+            best[j] = per[0].max()
+            multi = np.isfinite(per[1]) if len(per) > 1 else np.zeros(per.shape[1], bool)
+            second[j] = per[1][multi].min() if multi.any() else np.inf
+    return best, second
 
 
 # ---------------------------------------------------------------------------------------------------------------------
