@@ -111,11 +111,31 @@ int mbd_weighted_sum_runs(const float* weights_dev, const float* Y0s_dev, int n_
 int mbd_weighted_sqerr_sum(const float* weights_dev, const float* Y0s_dev, const float* mu_dev, int n_local, int HNu,
                            float* scratch_dev, float* partial_dev, mbd_stream s);
 
-/* Test hook: element-wise MBD_DIV (op 0), MBD_RCP (1), MBD_SQRT (2), mbd_atan2f (3) — the branch-free
- * exact device sequences of include/mbd_fp32.h — so tests can compare them with IEEE results bit for bit; and the
- * packed rollout kernel's atan2_ (csrc/pk_scalar.cuh): its scalar instantiation (4) and its two-lane f2 instantiation with
- * element i in the low (5) or the high (6) half, element n-1-i in the other. */
+/* Test hook: the device build of the fp32 math specification, element-wise, so tests can compare it with float64 and with
+ * the host build.  Ops: MBD_DIV (0), MBD_RCP (1), MBD_SQRT (2), mbd_atan2f (3) — the branch-free exact device sequences of
+ * include/mbd_fp32.h — and the packed rollout kernel's atan2_ (csrc/pk_scalar.cuh): its scalar instantiation (4) and its
+ * two-lane f2 instantiation with element i in the low (5) or the high (6) half, element n-1-i in the other;
+ * mbd_logf (7), mbd_expf (8), the sine (9) and the cosine (10) of mbd_sincosf, mbd_erfinvf (11), mbd_bits_to_normal of a's
+ * bits (12), mbd_tanhf (13), mbd_softplusf (14), mbd_swishf (15);  the packed kernel's scalar rcp_ (16), div_ (17),
+ * div_nn_ (18), sqrt_ (19) and the low / high halves of their two-lane forms, paired like ops 5 and 6: rcp_ (20 / 21),
+ * div_ (22 / 23), div_nn_ (24 / 25), sqrt_ (26 / 27);  and planted mistakes that exist only here, each a spec function
+ * with one step removed: the sine without its third Cody-Waite constant (28), mbd_expf without its second (29), rcp as the
+ * bare rcp.approx seed (30), sqrt without its final FMA (31), a division returning a * r after one Newton step (32). */
 int mbd_test_arith(int op, const float* a_dev, const float* b_dev, float* out_dev, int n, mbd_stream s);
+
+/* Test hook: err_dev[i] (double) = the error of op (as mbd_test_arith) at (a[i], b[i]) against a float64 reference from
+ * CUDA's double libm, in metric (u = 2^-24): ulps of fl(ref) (0), u |ref| (1), u (1 + |ref|) (2), u absolute (3), u |a| (4),
+ * exact: 0 when the result has the bits of fl(ref), else its distance in ulps and at least 1 (5), atan2 composed with the
+ * rounding of its quotient (6).  Metrics 1-4 forgive 2^-149 where |ref| < 2^-126.  The reference of a division, reciprocal
+ * or square root is the double operation, so fl(ref) is the correctly rounded float result. */
+int mbd_test_err(int op, int metric, const float* a_dev, const float* b_dev, double* err_dev, int n, mbd_stream s);
+
+/* Test hook: op and metric as mbd_test_err over the floats with bits first_bits + k * stride, k < count (uint32
+ * arithmetic), with `other` as the other operand (the first one when other_first).  Writes per block (nblocks of 256
+ * threads) the largest error (-1 for a block without inputs), the bits of the first input reaching it and the number of
+ * inputs with a nonzero error; the reduction order is fixed, so the result is deterministic. */
+int mbd_test_sweep(int op, int metric, uint32_t first_bits, uint32_t count, uint32_t stride, float other, int other_first,
+                   int nblocks, double* err_dev, uint32_t* bits_dev, uint32_t* cnt_dev, mbd_stream s);
 
 /* Ybar = tree-sum of the P rank partials; then score / Yim1 / Ybar_im1 literally as
  * mbd_planner.py:100,130-133.  coef = {sqrt(ab_i), 1/(1-ab_i), 1-ab_i, 1/sqrt(alpha_i), sqrt(ab_{i-1})}. */

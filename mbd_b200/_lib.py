@@ -182,6 +182,9 @@ def lib():
     L.mbd_weighted_sum_runs.argtypes = [c_vp, c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp]
     L.mbd_weighted_sqerr_sum.argtypes = [c_vp, c_vp, c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp]
     L.mbd_test_arith.argtypes = [ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_int, c_vp]
+    L.mbd_test_err.argtypes = [ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_int, c_vp]
+    L.mbd_test_sweep.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_float,
+                                 ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, c_vp]
     L.mbd_update.argtypes = [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_f32p, c_vp, c_vp]
     L.mbd_step_launch.argtypes = [ctypes.POINTER(StepPlan), c_vp]
     L.mbd_step_tail_launch.argtypes = [ctypes.POINTER(StepPlan), c_vp]
@@ -232,7 +235,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

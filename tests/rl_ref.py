@@ -27,14 +27,15 @@ from tests.xpbd_ref import ETA, R, U, exact_scale, fsum, gamma
 f32 = np.float32
 
 # ---- the fp32 functions (include/mbd_fp32.h, include/mbd_ppo.h) -------------------------------------------------------------
-EXP_REL = 2.0          # |mbd_expf(x) / exp(x) - 1| <= EXP_REL u on [-87, 88]; measured 1.51 / 1.44, test_fp32_spec.py::test_log_exp,
-                       # ::test_exp_positive
-LOG_REL = 2.0          # |mbd_logf(x) - log x| <= LOG_REL u |log x| on [e^-17, 2e6]; measured 1.43, ::test_log_scale_range
-TANH_ABS = 2.5         # |mbd_tanhf(x) - tanh x| <= TANH_ABS u (1 + |tanh x|); measured 2.00, ::test_rl_composites.  Absolute:
-                       # 1 - 2 / (e + 1) has no relative accuracy near 0
-SOFTPLUS = 1.5         # |mbd_softplusf(x) - softplus x| <= SOFTPLUS u (1 + softplus x); measured 1.07, ::test_rl_composites.
-                       # Absolute below 0: log(1 + e) keeps e to u only, and loses it below x ~ -17
-SWISH_REL = 3.5        # |mbd_swishf(x) - swish x| <= SWISH_REL u |swish x| for x >= -80; measured 2.80, ::test_rl_composites
+# The "max" figures are the exhaustive maxima over every float32 of the range on the device build
+# (tests/test_fp32_device_gpu.py, which proves each constant there); test_fp32_spec.py samples the host build.
+EXP_REL = 2.0          # |mbd_expf(x) / exp(x) - 1| <= EXP_REL u on [-87, 88]; max 1.540 at 70.35456 (0x428cb589)
+LOG_REL = 2.0          # |mbd_logf(x) - log x| <= LOG_REL u |log x| on [e^-17, 2e6]; max 1.548 at 0.7069994 (0x3f34fdea)
+TANH_ABS = 2.5         # |mbd_tanhf(x) - tanh x| <= TANH_ABS u (1 + |tanh x|); max 1.999 at -1.725e-4 (0xb934e004), 0 beyond
+                       # |x| = 30.  Absolute: 1 - 2 / (e + 1) has no relative accuracy near 0
+SOFTPLUS = 1.5         # |mbd_softplusf(x) - softplus x| <= SOFTPLUS u (1 + softplus x) on |x| <= 1e4; max 1.150 at 0.5456511
+                       # (0x3f0bafcb).  Absolute below 0: log(1 + e) keeps e to u only, and loses it below x ~ -17
+SWISH_REL = 3.5        # |mbd_swishf(x) - swish x| <= SWISH_REL u |swish x| for x in [-80, 1e5]; max 2.926 at -16.651403 (0xc1853613)
 SWISH_CAP = -80.0      # below it exp(-x) is capped at exp(80): |error| <= 1.01 |x| e^-80 (proven: both are below |x| e^-80 (1 + 4u))
 SWISH_LIP = 1.0999     # proven: sup |d/dx x sigma(x)| = 1.0998
 HALF_LOG_2PI = 0.5 * math.log(2 * math.pi)

@@ -15,8 +15,8 @@ Error model, u = 2^-24:
 * `rotate(v, q)` is charged (4.5 |q.r| + 4 |q.r|^2) |v| for the quaternion's radius (the map is quadratic in q: a radial
   perturbation a q moves R(q) v by at most 4|a||v|, a tangential one t by 2|t||v|) and gamma_32 |v| for rounding, which covers both the matrix form and the
   v + 2s(u x v) + 2u x (u x v) form the kernels use;
-* `atan2` costs (x.r + y.r) / (hypot(x, y) - x.r - y.r) propagated plus ATAN2_ULP ulps (tests/test_fp32_spec.py proves
-  ATAN2_ULP for `mbd_atan2f` over the operand ranges the Euler extraction produces); `cos` costs COS_ABS_ERR;
+* `atan2` costs (x.r + y.r) / (hypot(x, y) - x.r - y.r) propagated plus ATAN2_ULP ulps (tests/test_fp32_device_gpu.py proves
+  ATAN2_ULP for `mbd_atan2f` on the device build for every quotient inside the device division's domain); `cos` costs COS_ABS_ERR;
 * `sqrt(x)` propagates min(x.r / sqrt(x), sqrt(x.r)): the derivative form, or the Hoelder form below x ~ x.r;
 * a normalised fp32 vector has components in [-1 - 8u, 1 + 8u]; every value is intersected with such an interval where one
   is known (`clip_interval`), which keeps a direction whose norm is not much larger than its radius finite.  Where the
@@ -46,8 +46,10 @@ from mbd_b200.model import blob as B
 
 U = 2.0 ** -24
 ETA = 2.0 ** -149
-ATAN2_ULP = 4.0          # max ulp error of mbd_atan2f; tests/test_fp32_spec.py::test_atan2 proves it
-COS_ABS_ERR = 2.5e-7     # max absolute error of mbd_sincosf on |x| <= 1200; tests/test_fp32_spec.py::test_sincos
+ATAN2_ULP = 4.0          # max ulp error of mbd_atan2f; tests/test_fp32_device_gpu.py::test_atan2_exhaustive proves it on the
+                         # device build for every quotient (max 2.454 with the quotient's rounding), test_fp32_spec.py samples the host
+COS_ABS_ERR = 2.5e-7     # max absolute error of mbd_sincosf on |x| <= 1200 (max 9.32e-8 over every float32 there,
+                         # tests/test_fp32_device_gpu.py::test_unary_exhaustive)
 EPS = float(np.float32(1e-6))   # XPBD regulariser (ORC_EPS default)
 ROT_GRAD = 4.5   # |d(R(q) v)/dq| <= (4|radial| + 2|tangential|) |v| <= sqrt(20) |v| near |q| = 1
 ROT_ROUND = 32
