@@ -330,11 +330,15 @@ typedef struct mbd_vec_plan {
   float* done_dev;
   float* truncation_dev;
   float* steps_dev;
+  const float* factors_dev;     /* xpbd envs: [B][2] model factors (friction, actuator gear) of every env: env b steps with every contact
+                                 * friction fl(mu * F[b][0]) and every actuator gear fl(gear * F[b][1]); NULL = the nominal model.  A
+                                 * non-NULL table for car2d / pushT is MBD_EINVAL. */
 } mbd_vec_plan;
 /* env.reset(keys[b]) for every env b (keys_dev [B][2] uint32), in the threefry layout of mbd_set_prng_layout: state, first_state, obs,
  * first_obs, reward (0, pushT its reward), done, truncation 0, steps 0. */
 int mbd_vec_reset(const mbd_vec_plan* plan, const uint32_t* keys_dev, mbd_stream s);
-/* one env step of every env with the actions in plan->actions_dev (launches (1) and (2) above) */
+/* one env step of every env with the actions in plan->actions_dev (launches (1) and (2) above); with factors_dev, launch (1) is the
+ * per-env-model instantiation of the same kernel choice */
 int mbd_vec_step(const mbd_vec_plan* plan, mbd_stream s);
 /* obs of the states the caller wrote into state_dev; first_state = state, first_obs = obs; reward, done, truncation, steps 0 */
 int mbd_vec_set_state(const mbd_vec_plan* plan, mbd_stream s);

@@ -68,7 +68,8 @@ class VecPlan(ctypes.Structure):
                 ("reset_dev", c_vp), ("obs_layout", ctypes.c_int32), ("done_rule", ctypes.c_int32), ("episode_length", ctypes.c_int32),
                 ("nq", ctypes.c_int32), ("nqd", ctypes.c_int32), ("nu", ctypes.c_int32),
                 ("state_dev", c_vp), ("next_state_dev", c_vp), ("first_state_dev", c_vp), ("actions_dev", c_vp), ("obs_dev", c_vp),
-                ("first_obs_dev", c_vp), ("reward_dev", c_vp), ("done_dev", c_vp), ("truncation_dev", c_vp), ("steps_dev", c_vp)]
+                ("first_obs_dev", c_vp), ("reward_dev", c_vp), ("done_dev", c_vp), ("truncation_dev", c_vp), ("steps_dev", c_vp),
+                ("factors_dev", c_vp)]
 
 
 class PpoPlan(ctypes.Structure):

@@ -109,11 +109,13 @@ __device__ __forceinline__ q4 vqmul_xy(float ax, float ay, q4 q) {
 }
 
 // one sphere-plane contact of link l: accumulates the position-level correction (dp, dq); returns dlambda and
-// the contact point for the velocity pass
+// the contact point for the velocity pass.  DR (the vector env's per-env model): the friction is mu_dr, the caller's product
+// fl(mu * f_mu) of the blob word and the env's friction factor, in the place of the blob word.
+template <bool DR = false>
 __device__ __forceinline__ void contact_position_plane(const ModelSmem& M, int l, int ci, float im, v3 p, q4 q, v3 p_prev, q4 q_prev,
-                                                       v3& dp, q4& dq, float& dl_out, v3& cp_out) {
+                                                       v3& dp, q4& dq, float& dl_out, v3& cp_out, float mu_dr = 0.0f) {
   const int base = MBD_F_CON0 + ci * MBD_CON_STRIDE;
-  const float radius = M.lf(base + 3, l), mu = M.lf(base + 4, l);
+  const float radius = M.lf(base + 3, l), mu = DR ? mu_dr : M.lf(base + 4, l);
   v3 centre = vadd(p, vrotate(M.l3(base, l), q));
   float dist = centre.z - radius;
   v3 cp = V3(centre.x, centre.y, centre.z - (radius + 0.5f * dist));  // pos = c - n (r + dist/2)
@@ -143,9 +145,11 @@ __device__ __forceinline__ void contact_position_plane(const ModelSmem& M, int l
   cp_out = cp;
 }
 
+template <bool DR = false>
 __device__ __forceinline__ void contact_velocity_plane(const ModelSmem& M, int l, int ci, float im, float inv_dt, float elasticity, v3 p,
-                                                       v3 v, v3 w, v3 v_before, v3 w_before, v3 cp, float dl, v3& dv, v3& dw) {
-  const float mu = M.lf(MBD_F_CON0 + ci * MBD_CON_STRIDE + 4, l);
+                                                       v3 v, v3 w, v3 v_before, v3 w_before, v3 cp, float dl, v3& dv, v3& dw,
+                                                       float mu_dr = 0.0f) {
+  const float mu = DR ? mu_dr : M.lf(MBD_F_CON0 + ci * MBD_CON_STRIDE + 4, l);
   v3 r = vsub(cp, p);
   v3 rel = vadd(v, vcross(w, r));
   float vn = rel.z;
@@ -255,9 +259,10 @@ __device__ __forceinline__ void load_step_consts(const ModelSmem& M, StepConsts&
 
 // One brax.positional.pipeline.step for the link owned by this lane.  tau[k] = gear*clip(act) of
 // the lane's dof k (actuator.to_tau), already resolved by the caller.  All 32 lanes must call.
-template <int CMAX>
+// DR: every contact's friction is fl(mu * f_mu) (the vector env's per-env model factor).
+template <int CMAX, bool DR = false>
 __device__ __forceinline__ void positional_step(const ModelSmem& M, const LaneCfg& c, const StepConsts& K,
-                                                LinkState& s, const float tau[MBD_MAXDOF]) {
+                                                LinkState& s, const float tau[MBD_MAXDOF], float f_mu = 1.0f) {
   const bool jointed = c.ndof > 0;
   const LinkState prev = s;  // x_i_prev
 
@@ -407,7 +412,10 @@ __device__ __forceinline__ void positional_step(const ModelSmem& M, const LaneCf
     const q4 q0 = s.q;
 #pragma unroll
     for (int ci = 0; ci < CMAX; ++ci)
-      if (ci < c.ncon) contact_position_plane(M, c.l, ci, c.inv_mass, p0, q0, prev.p, prev.q, dp, dq, dlam[ci], cpos[ci]);
+      if (ci < c.ncon) {
+        const float mu = DR ? M.lf(MBD_F_CON0 + ci * MBD_CON_STRIDE + 4, c.l) * f_mu : 0.0f;
+        contact_position_plane<DR>(M, c.l, ci, c.inv_mass, p0, q0, prev.p, prev.q, dp, dq, dlam[ci], cpos[ci], mu);
+      }
     s.p = vfma(dp, K.collide_scale, s.p);
     s.q = qnormalize(qadd(s.q, qscale(dq, 0.5f * K.collide_scale)));
   }
@@ -424,8 +432,11 @@ __device__ __forceinline__ void positional_step(const ModelSmem& M, const LaneCf
     const v3 v0 = s.v, w0 = s.w;
 #pragma unroll
     for (int ci = 0; ci < CMAX; ++ci)
-      if (ci < c.ncon)
-        contact_velocity_plane(M, c.l, ci, c.inv_mass, K.inv_dt, K.elasticity, s.p, v0, w0, v_before, w_before, cpos[ci], dlam[ci], dv, dw);
+      if (ci < c.ncon) {
+        const float mu = DR ? M.lf(MBD_F_CON0 + ci * MBD_CON_STRIDE + 4, c.l) * f_mu : 0.0f;
+        contact_velocity_plane<DR>(M, c.l, ci, c.inv_mass, K.inv_dt, K.elasticity, s.p, v0, w0, v_before, w_before, cpos[ci], dlam[ci],
+                                   dv, dw, mu);
+      }
     s.v = vadd(s.v, dv);
     s.w = vadd(s.w, dw);
   }

@@ -187,10 +187,10 @@ struct SyncNamed {
 };
 
 // One brax.positional.pipeline.step for (link = this warp, sample = this lane).
-// All threads of the CTA must call.
-template <int CMAX, class Sync>
+// All threads of the CTA must call.  DR: every contact's friction is fl(mu * f_mu) (the vector env's per-env model factor).
+template <int CMAX, bool DR = false, class Sync>
 __device__ __forceinline__ void positional_step_wpl(const ModelSmem& M, const WarpCfg& c, const WplSmem& S,
-                                                    Sync& Y, LinkState& s, const float tau[MBD_MAXDOF]) {
+                                                    Sync& Y, LinkState& s, const float tau[MBD_MAXDOF], float f_mu = 1.0f) {
   const bool jointed = c.ndof > 0;
   const bool has_parent = c.parent >= 0;
   const v3 p_prev = s.p;
@@ -384,7 +384,10 @@ __device__ __forceinline__ void positional_step_wpl(const ModelSmem& M, const Wa
 #pragma unroll
     for (int ci = 0; ci < CMAX; ++ci) {
       dlam[ci] = 0.0f; cpos[ci] = V3(0.0f, 0.0f, 0.0f);
-      if (ci < c.ncon) contact_position_plane(M, c.l, ci, M.lf(MBD_F_INV_MASS, c.l), p0, q0, p_prev, q_prev, dp, dq, dlam[ci], cpos[ci]);
+      if (ci < c.ncon) {
+        const float mu = DR ? M.lf(MBD_F_CON0 + ci * MBD_CON_STRIDE + 4, c.l) * f_mu : 0.0f;
+        contact_position_plane<DR>(M, c.l, ci, M.lf(MBD_F_INV_MASS, c.l), p0, q0, p_prev, q_prev, dp, dq, dlam[ci], cpos[ci], mu);
+      }
     }
     s.p = vfma(dp, M.hf(MBD_H_COLLIDE_SCALE), s.p);
     s.q = qnormalize(qadd(s.q, qscale(dq, 0.5f * M.hf(MBD_H_COLLIDE_SCALE))));
@@ -400,9 +403,11 @@ __device__ __forceinline__ void positional_step_wpl(const ModelSmem& M, const Wa
     const v3 v0 = s.v, w0 = s.w;
 #pragma unroll
     for (int ci = 0; ci < CMAX; ++ci)
-      if (ci < c.ncon)
-        contact_velocity_plane(M, c.l, ci, M.lf(MBD_F_INV_MASS, c.l), M.hf(MBD_H_INV_DT), M.hf(MBD_H_ELASTICITY), s.p, v0, w0, v_before,
-                               w_before, cpos[ci], dlam[ci], dv, dw);
+      if (ci < c.ncon) {
+        const float mu = DR ? M.lf(MBD_F_CON0 + ci * MBD_CON_STRIDE + 4, c.l) * f_mu : 0.0f;
+        contact_velocity_plane<DR>(M, c.l, ci, M.lf(MBD_F_INV_MASS, c.l), M.hf(MBD_H_INV_DT), M.hf(MBD_H_ELASTICITY), s.p, v0, w0,
+                                   v_before, w_before, cpos[ci], dlam[ci], dv, dw, mu);
+      }
     s.v = vadd(s.v, dv);
     s.w = vadd(s.w, dw);
   }

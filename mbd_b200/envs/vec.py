@@ -13,9 +13,14 @@ buffer is owned here and fixed, so a step can be captured in a CUDA graph:
 
 Each env class is the specification: reset / step / obs / done reproduce the host `env.reset` / `env.step` of one state (raw state
 and reward bit for bit, observations within one float32 ulp), see DESIGN.md §5e.
+
+The xpbd envs can step every env with its own friction and actuator strength (DESIGN.md §5k):
+
+    venv.set_model_factors(friction=f, gear=g)  # scalars or [B] arrays; env b is scaled_env(env, f[b], g[b])
 """
 from __future__ import annotations
 
+import copy
 import dataclasses
 import os
 from typing import Optional
@@ -24,6 +29,7 @@ import numpy as np
 import torch
 
 from .. import _lib, ops
+from ..model import blob as blob_mod
 from .ant import Ant
 from .base import PipelineEnv
 from .car2d import Car2d
@@ -137,6 +143,40 @@ def env_spec(env) -> _Spec:
     return _Spec(_lib.VEC_XPBD, layout, done, nq, nqd, sys.act_size(), len(env._links) * 13, nq - skip + nqd, rt)
 
 
+def factor_column(value, B: int, name: str) -> np.ndarray:
+    """a model factor as float32 [B]: a scalar (every env) or a [B] array; ValueError unless every value is finite and >= 0"""
+    if isinstance(value, torch.Tensor):
+        value = value.detach().cpu().numpy()
+    v = np.asarray(value, dtype=np.float64)
+    if v.ndim == 0:
+        v = np.full(B, v)
+    if v.shape != (B,):
+        raise ValueError(f"{name} must be a scalar or an array of shape ({B},) (got shape {v.shape})")
+    with np.errstate(over="ignore"):
+        f = v.astype(np.float32)
+    if not (np.isfinite(f).all() and (f >= 0).all()):
+        raise ValueError(f"{name} factors must be finite and >= 0 (got {v.tolist()})")
+    return f
+
+
+def scaled_env(env: PipelineEnv, friction: float = 1.0, gear: float = 1.0) -> PipelineEnv:
+    """the specification of a vector env stepped with model factors (friction, gear): a host env of the same class whose every
+    contact friction is fl(mu * friction) and every actuator gear fl(gear_a * gear), in float32 as the kernel forms them, with its
+    device model rebuilt from that `sys`.  Its blob differs from env's in exactly those words."""
+    if not isinstance(env, PipelineEnv):
+        raise ValueError(f"model factors exist for the xpbd envs only, not {type(env).__name__}")
+    fr, gr = factor_column(friction, 1, "friction")[0], factor_column(gear, 1, "gear")[0]
+    sys = env.sys
+    contacts = [dict(c, friction=float(np.float32(np.float32(c["friction"]) * fr))) for c in sys.contacts]
+    act_gear = np.array([float(np.float32(np.float32(g) * gr)) for g in sys.act_gear], dtype=np.float64)
+    out = copy.copy(env)
+    out.sys = dataclasses.replace(sys, contacts=contacts, act_gear=act_gear)
+    out.blob = blob_mod.pack(out.sys, out._n_frames, out.reward_kind, links=out._links, track_links=tuple(out.track_links),
+                             **out._pack_kwargs())
+    out._models = {}
+    return out
+
+
 @dataclasses.dataclass
 class VecState:
     """views on the VecEnv's buffers (overwritten by the next reset / step / set_state)"""
@@ -184,6 +224,25 @@ class VecEnv:
         for name in ("state", "next_state", "first_state", "actions", "obs", "first_obs", "reward", "done", "truncation", "steps"):
             setattr(P, name + "_dev", getattr(self, name).data_ptr())
         self.plan = P
+        self.factors: Optional[torch.Tensor] = None   # [B, 2] friction | gear factors once set_model_factors gave any
+
+    def set_model_factors(self, friction=None, gear=None) -> None:
+        """step env b with every contact friction scaled by friction[b] and every actuator gear by gear[b] (xpbd envs): env b then
+        steps as the nominal VecEnv of scaled_env(env, friction[b], gear[b]), bit for bit.  Each argument is a scalar or a [B]
+        array of finite values >= 0; an omitted one is 1.  Both omitted: the nominal model (the kernels of a VecEnv without
+        factors).  The [B, 2] table is written in place, so a captured graph keeps reading the current values."""
+        if self.spec.kind != _lib.VEC_XPBD:
+            raise ValueError("model factors exist for the positional (xpbd) envs only")
+        B = self.num_envs
+        fr = factor_column(1.0 if friction is None else friction, B, "friction")
+        gr = factor_column(1.0 if gear is None else gear, B, "gear")
+        if friction is None and gear is None:
+            self.plan.factors_dev = None
+            return
+        if self.factors is None:
+            self.factors = torch.empty((B, 2), device=self.device, dtype=torch.float32)
+        self.factors.copy_(torch.from_numpy(np.stack([fr, gr], axis=1)))
+        self.plan.factors_dev = self.factors.data_ptr()
 
     # ---- the batched env API -------------------------------------------------------------------------------------------------
     def _view(self) -> VecState:

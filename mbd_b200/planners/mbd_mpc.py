@@ -7,6 +7,9 @@ Nwarm ... 1 on the same schedule rows as the Ndiffuse-step solve, with the keys 
 `rng, rng_c = split(rng)`.  The first row of the plan, unclipped, is applied to the plant with `env.step` (no episode wrapper,
 `done` ignored).
 
+The plant may differ from the model the planner plans with (DESIGN.md §5k): `plant_friction` and `plant_gear` scale every contact
+friction and every actuator gear of the plant of one problem (`envs.vec.scaled_env`), while the planner keeps the nominal model.
+
 Everything runs on the device: B closed loops (one per seed) share one `BatchedDiffusionEngine` that plans from the state buffer of
 a `VecEnv`, and `mbd_mpc_advance` executes the plan and re-arms the next control step.  A warm control step (Nwarm batched
 diffusion steps, ACT, the env step, RECORD) is one captured CUDA graph:
@@ -15,6 +18,7 @@ diffusion steps, ACT, the env step, RECORD) is one captured CUDA graph:
 """
 from __future__ import annotations
 
+import math
 import os
 import time
 from dataclasses import dataclass
@@ -41,6 +45,9 @@ class Args(mbd_planner.Args):
     # receding horizon
     Nwarm: int = 10  # diffusion steps of every control step after the first (1 <= Nwarm <= Ndiffuse - 1)
     Nstep: int = 50  # control steps
+    # model mismatch: the plant's friction and actuator gear over the planner's (xpbd envs; per problem)
+    plant_friction: float = 1.0
+    plant_gear: float = 1.0
 
 
 # fields every problem of one run_mpc_batch call must share; seed, temp_sample, beta0 and betaT may differ
@@ -66,8 +73,27 @@ def check_args(args_list, batch: bool) -> None:
         vals = [getattr(a, f) for a in args_list]
         if any(v != vals[0] for v in vals):
             raise ValueError(f"run_mpc_batch: every problem must have the same {f} (got {vals})")
+    check_plant(args_list)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1 or (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
         raise ValueError("the controller runs on one GPU; it cannot run under WORLD_SIZE > 1")
+
+
+def check_plant(args_list) -> None:
+    """plant_friction / plant_gear: finite and >= 0, and 1 on car2d and pushT (ValueError)"""
+    for a in args_list:
+        for f in ("plant_friction", "plant_gear"):
+            v = getattr(a, f)
+            if not (math.isfinite(v) and v >= 0):
+                raise ValueError(f"{f} must be finite and >= 0 (got {v})")
+            if v != 1.0 and a.env_name in ("car2d", "pushT"):
+                raise ValueError(f"{f} != 1: model factors exist for the positional (xpbd) envs only, not {a.env_name}")
+
+
+def plant_factors(args_list):
+    """([B] friction, [B] gear) of the problems' plants, or None when every plant is the nominal model"""
+    fr = [float(a.plant_friction) for a in args_list]
+    gr = [float(a.plant_gear) for a in args_list]
+    return None if all(v == 1.0 for v in fr + gr) else (fr, gr)
 
 
 def mpc_keys(seed: int, Ndiffuse: int, Nwarm: int, Nstep: int):
@@ -131,13 +157,19 @@ class Controller:
         s0 = torch.stack([env_tensors(env, s, False, d)[2].reshape(-1) for s in self.host_states]).contiguous()
         self.S = s0.shape[1]
         self.venv = None
+        factors = plant_factors(args_list)
         if self.host:
+            from mbd_b200.envs.vec import scaled_env
             state_buffer = s0
+            # every problem's plant as a host env: the specification of the vector env's per-env model
+            self.plants = [env] * self.B if factors is None else [scaled_env(env, fr, gr) for fr, gr in zip(*factors)]
         else:
             from mbd_b200.envs.vec import VecEnv
             self.venv = VecEnv(env, self.B, device=d)
             if self.venv.state.shape[1] != self.S:
                 raise ValueError(f"the vector env's state has {self.venv.state.shape[1]} words, the planner's {self.S}")
+            if factors is not None:
+                self.venv.set_model_factors(friction=factors[0], gear=factors[1])
             self.venv.set_state(s0)
             state_buffer = self.venv.state
         self.engine = self._make_engine(colds, state_buffer)
@@ -268,7 +300,7 @@ class Controller:
                 a = P[:, 0].cpu().numpy()
                 rh[:, c] = e.rew_hist[:, 1].cpu().numpy()
                 for b in range(B):
-                    st[b] = env.step(st[b], a[b])
+                    st[b] = self.plants[b].step(st[b], a[b])
                     sts[b, c + 1] = host_raw(env, st[b])
                     rews[b, c] = np.float32(st[b].reward)
                 acts[:, c] = a

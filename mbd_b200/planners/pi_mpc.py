@@ -10,7 +10,8 @@ place of Ndiffuse).  Execute, shift and the result are mbd_mpc.py's.
 The sampling sigma is **reset, not carried**: every control step c >= 1 starts from `sigma_warm`.  MPPI and CEM keep it; CMA-ES
 adapts it inside the control step as the reference's update does, and the sigma each control step ends with is logged
 (`MpcResult.sigmas`).  A carried CMA-ES sigma would sit at the reference's 1e-3 floor after the first solve and could not re-plan.
-With `sigma_warm = 1.0` a warm step is the reference's update verbatim.
+With `sigma_warm = 1.0` a warm step is the reference's update verbatim.  `plant_friction` / `plant_gear` give every problem its
+own plant, as in mbd_mpc.py.
 
 Everything runs on the device: the B loops share one `BatchedPathIntegralEngine` that plans from the state buffer of a `VecEnv`,
 `mbd_mpc_pi_advance` executes the plan, re-arms the next control step and resets its sigma rows, and a warm control step (Nwarm
@@ -40,6 +41,9 @@ class Args(path_integral.Args):
     Nwarm: int = 10  # refinement steps of every control step after the first (1 <= Nwarm <= Nrefine - 1)
     Nstep: int = 50  # control steps
     sigma_warm: float = 1.0  # the sampling sigma every control step after the first starts from
+    # model mismatch (mbd_mpc.Args): the plant's friction and actuator gear over the planner's (xpbd envs; per problem)
+    plant_friction: float = 1.0
+    plant_gear: float = 1.0
 
 
 # fields every problem of one run_pi_mpc_batch call must share; seed and temp_sample may differ
@@ -66,6 +70,7 @@ def check_args(args_list, batch: bool) -> None:
         vals = [getattr(a, f) for a in args_list]
         if any(v != vals[0] for v in vals):
             raise ValueError(f"run_pi_mpc_batch: every problem must have the same {f} (got {vals})")
+    mbd_mpc.check_plant(args_list)
     import torch.distributed as dist
     if int(os.environ.get("WORLD_SIZE", "1")) > 1 or (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
         raise ValueError("the controller runs on one GPU; it cannot run under WORLD_SIZE > 1")

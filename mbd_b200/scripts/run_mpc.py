@@ -7,6 +7,8 @@ For each of mbd, mppi, cma-es and cem the eight seeds run as ONE batch of recedi
 run_pi_mpc_batch) at the same Nsample, Hsample, Nwarm and Nstep, the cold solve at Nsolve steps (Ndiffuse = Nrefine) and each
 planner's recommended temperature for the env.  `zero` is the plant under zero actions from the same reset states.  Per algorithm
 one line: the closed-loop mean reward over the seeds and the wall time of one warm control step of the whole batch.
+`--plant_friction` / `--plant_gear` run every algorithm and the zero-action baseline against a plant whose contact friction and
+actuator gear are scaled by those factors, while the planners keep the nominal model (DESIGN.md §5k).
 """
 from __future__ import annotations
 
@@ -31,12 +33,15 @@ class Args:
     Nwarm: int = 10  # steps of every later control step
     Nstep: int = 50  # control steps
     sigma_warm: float = 1.0  # the baselines' sampling sigma at the start of every warm control step
+    plant_friction: float = 1.0  # the plant's contact friction over the planners' model (xpbd envs)
+    plant_gear: float = 1.0  # the plant's actuator gear over the planners' model (xpbd envs)
 
 
 def mbd_args(args: Args, seeds=SEEDS):
     temp = mbd_planner.TEMP_RECOMMEND.get(args.env_name, mbd_planner.Args.temp_sample)
     return [mbd_mpc.Args(seed=s, env_name=args.env_name, Nsample=args.Nsample, Hsample=args.Hsample, Ndiffuse=args.Nsolve,
-                         Nwarm=args.Nwarm, Nstep=args.Nstep, temp_sample=temp, not_render=True, disable_recommended_params=True)
+                         Nwarm=args.Nwarm, Nstep=args.Nstep, temp_sample=temp, plant_friction=args.plant_friction,
+                         plant_gear=args.plant_gear, not_render=True, disable_recommended_params=True)
             for s in seeds]
 
 
@@ -44,13 +49,17 @@ def pi_args(args: Args, method: str, seeds=SEEDS):
     temp = path_integral.TEMP_RECOMMEND.get(args.env_name, path_integral.Args.temp_sample)
     return [pi_mpc.Args(seed=s, env_name=args.env_name, update_method=method, Nsample=args.Nsample, Hsample=args.Hsample,
                         Nrefine=args.Nsolve, Nwarm=args.Nwarm, Nstep=args.Nstep, sigma_warm=args.sigma_warm, temp_sample=temp,
-                        not_render=True, disable_recommended_params=True) for s in seeds]
+                        plant_friction=args.plant_friction, plant_gear=args.plant_gear, not_render=True,
+                        disable_recommended_params=True) for s in seeds]
 
 
-def zero_action_rewards(env, states0: np.ndarray, Nstep: int) -> np.ndarray:
-    """[B] mean reward of Nstep env steps under zero actions from states0 [B, S] (the controller's plant: no episode wrapper)"""
+def zero_action_rewards(env, states0: np.ndarray, Nstep: int, friction=1.0, gear=1.0) -> np.ndarray:
+    """[B] mean reward of Nstep env steps under zero actions from states0 [B, S] (the controller's plant: no episode wrapper, model
+    factors friction / gear, scalars or [B])"""
     from mbd_b200.envs.vec import VecEnv
     venv = VecEnv(env, len(states0))
+    if np.any(np.asarray(friction) != 1.0) or np.any(np.asarray(gear) != 1.0):
+        venv.set_model_factors(friction=friction, gear=gear)
     venv.set_state(states0)
     zeros = torch.zeros_like(venv.actions)
     rews = torch.stack([venv.step(zeros).reward.clone() for _ in range(Nstep)], dim=1)
@@ -78,7 +87,8 @@ def main(argv=None):
         out[algo] = res.reward
         print(f"{algo}: rew: {res.reward.mean():.2f} \\pm {res.reward.std():.2f}  time per control step: {per * 1e3:.2f} ms "
               f"(batch of {len(res.reward)})")
-    zero = zero_action_rewards(mbd_b200.envs.get_env(args.env_name), res.states[:, 0], args.Nstep)   # s_0 is every algorithm's
+    zero = zero_action_rewards(mbd_b200.envs.get_env(args.env_name), res.states[:, 0], args.Nstep,   # s_0 is every algorithm's
+                               args.plant_friction, args.plant_gear)
     out["zero"] = zero
     print(f"zero: rew: {zero.mean():.2f} \\pm {zero.std():.2f}")
     return out
