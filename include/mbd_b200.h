@@ -197,7 +197,20 @@ typedef struct mbd_step_plan {
   const uint64_t* peer_base_ptrs;    /* host array [P]: base address of every rank's symmetric buffer (NULL when P == 1) */
   uint64_t off_rews_words, off_logpd_words, off_partial_words, off_flags_words;  /* flags: 2 rows of 8 words, zeroed */
   uint64_t timeout_cycles;           /* cross-GPU rendezvous timeout in SM cycles; 0 = default (~20 s) */
+  /* planner ensemble (appended; mbd_batch_step_launch / mbd_pi_batch_step_launch only, xpbd envs, DESIGN.md §5l).  Problem b
+   * rolls every sample Y_bn out under ens_k models (f_bk, g_bk): every contact friction fl(mu * f_bk), every actuator gear
+   * fl(gear * g_bk).  ens_rews[b][n][k] receives each member return r_bnk; the sample return the tail reads is
+   * rews[b][n] = fl(fl(fl(r_bn0 + r_bn1) + ...) / ens_k), summed in member order.  NULL / 0 = today's step. */
+  const float* ens_factors_dev;      /* [B][ens_k][2]: friction factor, gear factor of every member of every problem */
+  float* ens_rews_dev;               /* [B][N][ens_k] */
+  int32_t ens_k;                     /* members per problem, 1 .. MBD_ENS_MAXK with a table, 0 without */
+  int32_t ens_pad;
 } mbd_step_plan;
+#define MBD_ENS_MAXK 16
+/* sizeof(mbd_step_plan), offsetof ens_factors_dev / ens_rews_dev / ens_k and MBD_ENS_MAXK (cross-checked against the ctypes mirror) */
+int mbd_ens_abi_sizes(int32_t* out, int n);
+/* mbd_step_launch, mbd_step_launch_ev and mbd_step_tail_launch refuse an ensemble (MBD_EINVAL): the single-solve, sharded and
+ * benchmark step keep their three launches. */
 int mbd_step_launch(const mbd_step_plan* plan, mbd_stream s);
 /* B independent solves of one env and shape in lockstep: three launches, graph-capturable.  Every per-problem buffer of
  * `plan` holds B consecutive single-problem blocks (state_init [B][state], params [B][Ndiffuse], ctl [B],
@@ -206,7 +219,12 @@ int mbd_step_launch(const mbd_step_plan* plan, mbd_stream s);
  * temps_dev [B] or NULL (= plan->temp for every problem).  car_params / xref are shared by all problems.  Problem b draws
  * the noise of a stand-alone solve with its own key and reduces in the same order, so it reproduces mbd_step_launch on
  * its own buffers bit for bit.  MBD_EINVAL (with mbd_last_error) before any CUDA call for B < 1, P != 1, Ndiffuse < 2 or
- * a plan mbd_step_launch would refuse. */
+ * a plan mbd_step_launch would refuse.
+ * With a planner ensemble (ens_factors_dev) launch (1) becomes three launches: the batched sampler (the fused kernels' Y0s bits),
+ * the ensemble rollout (rollout slot s of problem b is sample s / ens_k under member s % ens_k) and the ordered member mean into
+ * rews; launches (2) and (3) follow unchanged.  MBD_EINVAL before any CUDA call for a table without ens_rews or ens_rews without a
+ * table, ens_k outside 1 .. MBD_ENS_MAXK with a table or not 0 without one, a flat-state env (model NULL), a demo (xref) or
+ * B * N * ens_k >= 2^31. */
 int mbd_batch_step_launch(const mbd_step_plan* plan, int B, int Ndiffuse, const float* temps_dev, mbd_stream s);
 /* ---- the path-integral baselines (upstream mbd/planners/path_integral.py:33-52) as the same three launches ----------------
  * B independent refinements of one env and shape in lockstep, laid out exactly as mbd_batch_step_launch (Ndiffuse = Nrefine
@@ -225,7 +243,8 @@ typedef struct mbd_pi_bufs {        /* 24 bytes */
   float* cma_scratch_dev;           /* CMA-ES: [B][ceil(N/64) + 1][H*Nu] (NULL otherwise) */
   int32_t* cem_idx_dev;             /* CEM: [B][MBD_PI_IDX_STRIDE] (NULL otherwise) */
 } mbd_pi_bufs;
-/* tail_only != 0: launches (2) and (3) only, on whatever the caller put into Y0s / rews / Ybars[i] / params[i] (tests).
+/* tail_only != 0: launches (2) and (3) only, on whatever the caller put into Y0s / rews / Ybars[i] / params[i] (tests); it ignores
+ * the ensemble fields.  Otherwise a planner ensemble runs launch (1) as mbd_batch_step_launch does.
  * MBD_EINVAL (with mbd_last_error) before any CUDA call for an unknown method, P != 1, Nrefine < 2, B outside 1..65535, a demo
  * (xref), a missing buffer of the method, or a plan mbd_batch_step_launch would refuse. */
 int mbd_pi_batch_step_launch(const mbd_step_plan* plan, int B, int Nrefine, int method, const float* temps_dev,

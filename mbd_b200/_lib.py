@@ -42,6 +42,7 @@ class StepPlan(ctypes.Structure):
         ("peer_base_ptrs", ctypes.POINTER(ctypes.c_uint64)),
         ("off_rews_words", ctypes.c_uint64), ("off_logpd_words", ctypes.c_uint64), ("off_partial_words", ctypes.c_uint64),
         ("off_flags_words", ctypes.c_uint64), ("timeout_cycles", ctypes.c_uint64),
+        ("ens_factors_dev", c_vp), ("ens_rews_dev", c_vp), ("ens_k", ctypes.c_int32), ("ens_pad", ctypes.c_int32),
     ]
 
 
@@ -140,6 +141,7 @@ BBO_FNS = {"Ackley": 1, "Rastrigin": 2, "Levy": 3}   # MBD_BBO_ACKLEY / MBD_BBO_
 PI_METHODS = {"mppi": 1, "cma-es": 2, "cem": 3}   # MBD_PI_MPPI / MBD_PI_CMAES / MBD_PI_CEM
 PI_IDX_STRIDE = 16       # MBD_PI_IDX_STRIDE: ints per problem in cem_idx (10 picks, then the count)
 PI_TOPK = 10
+ENS_MAXK = 16            # MBD_ENS_MAXK: members of a planner ensemble
 
 STEP_PARAMS_WORDS = 8    # sizeof(mbd_step_params) / 4
 STEP_CTL_WORDS = 32      # sizeof(mbd_step_ctl) / 4
@@ -193,6 +195,7 @@ def lib():
     L.mbd_pi_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
                                            ctypes.POINTER(PiBufs), ctypes.c_int, c_vp]
     L.mbd_pi_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_ens_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_bbo_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
                                             ctypes.POINTER(BboBufs), c_vp]
     L.mbd_bbo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
@@ -236,7 +239,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_ens_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

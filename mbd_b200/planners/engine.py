@@ -104,6 +104,26 @@ def env_tensors(env, state_init, enable_demo: bool, d: torch.device):
     raise ValueError(env.kind)
 
 
+def ensemble_table(table, B: int, env, enable_demo: bool) -> np.ndarray:
+    """a planner ensemble as the float32 [B, K, 2] table of mbd_step_plan.ens_factors_dev: table[b][k] = (friction factor, gear
+    factor) of member k of problem b, member-major within each problem.  ValueError unless the env is positional (xpbd), there is no
+    demo, the shape is [B, K, 2] with 1 <= K <= ENS_MAXK and every value is finite and >= 0 in float32."""
+    if getattr(env, "kind", None) != "xpbd":
+        raise ValueError(f"planner ensembles exist for the positional (xpbd) envs only, not {type(env).__name__}")
+    if enable_demo:
+        raise ValueError("a planner ensemble has no demonstration (enable_demo must be False)")
+    if isinstance(table, torch.Tensor):
+        table = table.detach().cpu().numpy()
+    t = np.asarray(table, dtype=np.float64)
+    if t.ndim != 3 or t.shape[0] != B or t.shape[2] != 2 or not 1 <= t.shape[1] <= _lib.ENS_MAXK:
+        raise ValueError(f"the ensemble must have shape ({B}, K, 2) with 1 <= K <= {_lib.ENS_MAXK} (got {t.shape})")
+    with np.errstate(over="ignore"):
+        f = np.ascontiguousarray(t.astype(np.float32))
+    if not (np.isfinite(f).all() and (f >= 0).all()):
+        raise ValueError(f"ensemble factors must be finite and >= 0 (got {t.reshape(-1).tolist()})")
+    return f
+
+
 def xref_len(env, xref) -> int:
     """href of the step plan: the demonstration's length in steps (0 without one)"""
     return 0 if xref is None else int(xref.shape[1] if env.kind == "xpbd" else xref.shape[0])
@@ -324,14 +344,22 @@ class BatchedDiffusionEngine:
 
     state_buffer: an external [B, S] float32 device tensor the steps read the initial states from instead of the engine's own copy
     of `state_inits` (the receding-horizon controller passes `VecEnv.state`, so every step plans from the plant's current state).
-    Its layout must be the engine's; its content is the caller's (`state_inits` then only fix the layout)."""
+    Its layout must be the engine's; its content is the caller's (`state_inits` then only fix the layout).
+
+    ensemble: a planner ensemble [B][K][2] (DESIGN.md §5l, positional envs, no demo): problem b rolls every sample out under the K
+    models (friction ensemble[b][k][0], gear ensemble[b][k][1]) and the tail reads the mean of the K returns.  `ens_rews` [B, N, K]
+    holds every member return of the last step.  None: today's step."""
+
+    ens_factors: Optional[torch.Tensor] = None   # [B, K, 2] on the device once an ensemble is given
+    ens_rews: Optional[torch.Tensor] = None      # [B, N, K]
 
     def __init__(self, env, Nsample: int, Hsample: int, temps, enable_demo: bool, state_inits, Ndiffuse: int,
-                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None):
+                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None):
         self.env = env
         self.B = len(state_inits)
         if self.B < 1 or len(temps) != self.B:
             raise ValueError(f"{self.B} initial states and {len(temps)} temperatures: need one of each per problem, B >= 1")
+        ens = None if ensemble is None else ensemble_table(ensemble, self.B, env, enable_demo)
         self.N, self.H = int(Nsample), int(Hsample)
         self.enable_demo = bool(enable_demo)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -352,6 +380,21 @@ class BatchedDiffusionEngine:
             self.state_init = state_buffer
         self.rew_xref = float(getattr(env, "rew_xref", 0.0))
         self._alloc(temps)
+        if ens is not None:
+            K = ens.shape[1]
+            self.ens_factors = torch.from_numpy(ens).to(self.device)
+            self.ens_rews = torch.empty((self.B, self.N, K), device=self.device, dtype=torch.float32)
+            p = self._plan_c
+            p.ens_factors_dev, p.ens_rews_dev, p.ens_k = self.ens_factors.data_ptr(), self.ens_rews.data_ptr(), K
+
+    def set_ensemble(self, table):
+        """rewrites the planner ensemble in place (same B and K): a captured step reads the new values on its next replay"""
+        if self.ens_factors is None:
+            raise ValueError("this engine was built without a planner ensemble")
+        ens = ensemble_table(table, self.B, self.env, self.enable_demo)
+        if ens.shape != tuple(self.ens_factors.shape):
+            raise ValueError(f"the ensemble must keep its shape {tuple(self.ens_factors.shape)} (got {ens.shape})")
+        self.ens_factors.copy_(torch.from_numpy(ens))
 
     def _alloc(self, temps):
         """the per-problem device buffers and the C plan, from B, N, HNu, Nd, enable_demo and the env tensors set before"""

@@ -9,6 +9,8 @@ Nwarm ... 1 on the same schedule rows as the Ndiffuse-step solve, with the keys 
 
 The plant may differ from the model the planner plans with (DESIGN.md §5k): `plant_friction` and `plant_gear` scale every contact
 friction and every actuator gear of the plant of one problem (`envs.vec.scaled_env`), while the planner keeps the nominal model.
+The planner may plan against an ensemble of models instead (DESIGN.md §5l): with `plan_friction` / `plan_gear` of length K every
+sample is rolled out under the K models (plan_friction[k], plan_gear[k]) and scored by the mean of the K returns.
 
 Everything runs on the device: B closed loops (one per seed) share one `BatchedDiffusionEngine` that plans from the state buffer of
 a `VecEnv`, and `mbd_mpc_advance` executes the plan and re-arms the next control step.  A warm control step (Nwarm batched
@@ -48,6 +50,10 @@ class Args(mbd_planner.Args):
     # model mismatch: the plant's friction and actuator gear over the planner's (xpbd envs; per problem)
     plant_friction: float = 1.0
     plant_gear: float = 1.0
+    # planner ensemble: member k plans with friction plan_friction[k] and gear plan_gear[k] (xpbd envs; equal lengths K, the same K
+    # for every problem of a batch, values per problem); empty = the nominal model
+    plan_friction: tuple[float, ...] = ()
+    plan_gear: tuple[float, ...] = ()
 
 
 # fields every problem of one run_mpc_batch call must share; seed, temp_sample, beta0 and betaT may differ
@@ -74,6 +80,7 @@ def check_args(args_list, batch: bool) -> None:
         if any(v != vals[0] for v in vals):
             raise ValueError(f"run_mpc_batch: every problem must have the same {f} (got {vals})")
     check_plant(args_list)
+    check_plan(args_list)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1 or (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
         raise ValueError("the controller runs on one GPU; it cannot run under WORLD_SIZE > 1")
 
@@ -87,6 +94,36 @@ def check_plant(args_list) -> None:
                 raise ValueError(f"{f} must be finite and >= 0 (got {v})")
             if v != 1.0 and a.env_name in ("car2d", "pushT"):
                 raise ValueError(f"{f} != 1: model factors exist for the positional (xpbd) envs only, not {a.env_name}")
+
+
+def check_plan(args_list) -> None:
+    """plan_friction / plan_gear: equal lengths K <= ENS_MAXK, the same K for every problem, values finite and >= 0, and empty on
+    car2d and pushT (ValueError)"""
+    ks = set()
+    for a in args_list:
+        fr, gr = tuple(a.plan_friction), tuple(a.plan_gear)
+        if len(fr) != len(gr):
+            raise ValueError(f"plan_friction and plan_gear must have the same length (got {len(fr)} and {len(gr)})")
+        if len(fr) > _lib.ENS_MAXK:
+            raise ValueError(f"a planner ensemble has at most {_lib.ENS_MAXK} members (got {len(fr)})")
+        if fr and a.env_name in ("car2d", "pushT"):
+            raise ValueError(f"planner ensembles exist for the positional (xpbd) envs only, not {a.env_name}")
+        for f, vals in (("plan_friction", fr), ("plan_gear", gr)):
+            with np.errstate(over="ignore"):
+                v32 = np.asarray(vals, dtype=np.float64).astype(np.float32)
+            if not (np.isfinite(v32).all() and (v32 >= 0).all()):
+                raise ValueError(f"{f} must be finite and >= 0 in float32 (got {vals})")
+        ks.add(len(fr))
+    if len(ks) > 1:
+        raise ValueError(f"every problem of a batch must plan with the same number of ensemble members (got {sorted(ks)})")
+
+
+def plan_ensemble(args_list):
+    """the [B, K, 2] planner ensemble of the problems (member k of problem b = (plan_friction[k], plan_gear[k])), or None when
+    they plan with the nominal model"""
+    if not args_list[0].plan_friction:
+        return None
+    return np.array([[(f, g) for f, g in zip(a.plan_friction, a.plan_gear)] for a in args_list], dtype=np.float32)
 
 
 def plant_factors(args_list):
@@ -194,7 +231,7 @@ class Controller:
             print(f"init sigma = {sigmas[-1]:.2e}")
             scheds.append((sigmas, alphas, alphas_bar))
         e = BatchedDiffusionEngine(self.env, a0.Nsample, a0.Hsample, [a.temp_sample for a in self.args], False, self.host_states,
-                                   a0.Ndiffuse, device=self.device, state_buffer=state_buffer)
+                                   a0.Ndiffuse, device=self.device, state_buffer=state_buffer, ensemble=plan_ensemble(self.args))
         e.load_schedule(colds, [s[0] for s in scheds], [s[1] for s in scheds], [s[2] for s in scheds])
         return e
 

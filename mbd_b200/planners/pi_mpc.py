@@ -11,7 +11,7 @@ The sampling sigma is **reset, not carried**: every control step c >= 1 starts f
 adapts it inside the control step as the reference's update does, and the sigma each control step ends with is logged
 (`MpcResult.sigmas`).  A carried CMA-ES sigma would sit at the reference's 1e-3 floor after the first solve and could not re-plan.
 With `sigma_warm = 1.0` a warm step is the reference's update verbatim.  `plant_friction` / `plant_gear` give every problem its
-own plant, as in mbd_mpc.py.
+own plant and `plan_friction` / `plan_gear` a planner ensemble, as in mbd_mpc.py.
 
 Everything runs on the device: the B loops share one `BatchedPathIntegralEngine` that plans from the state buffer of a `VecEnv`,
 `mbd_mpc_pi_advance` executes the plan, re-arms the next control step and resets its sigma rows, and a warm control step (Nwarm
@@ -44,6 +44,9 @@ class Args(path_integral.Args):
     # model mismatch (mbd_mpc.Args): the plant's friction and actuator gear over the planner's (xpbd envs; per problem)
     plant_friction: float = 1.0
     plant_gear: float = 1.0
+    # planner ensemble (mbd_mpc.Args): member k plans with (plan_friction[k], plan_gear[k]); empty = the nominal model
+    plan_friction: tuple[float, ...] = ()
+    plan_gear: tuple[float, ...] = ()
 
 
 # fields every problem of one run_pi_mpc_batch call must share; seed and temp_sample may differ
@@ -71,6 +74,7 @@ def check_args(args_list, batch: bool) -> None:
         if any(v != vals[0] for v in vals):
             raise ValueError(f"run_pi_mpc_batch: every problem must have the same {f} (got {vals})")
     mbd_mpc.check_plant(args_list)
+    mbd_mpc.check_plan(args_list)
     import torch.distributed as dist
     if int(os.environ.get("WORLD_SIZE", "1")) > 1 or (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
         raise ValueError("the controller runs on one GPU; it cannot run under WORLD_SIZE > 1")
@@ -90,7 +94,8 @@ class Controller(mbd_mpc.Controller):
         a0 = self.args[0]
         self.sigmas = torch.zeros((self.B, self.Nstep), device=self.device, dtype=torch.float32)
         e = BatchedPathIntegralEngine(self.env, a0.Nsample, a0.Hsample, [a.temp_sample for a in self.args], self.host_states,
-                                      a0.Nrefine, a0.update_method, device=self.device, state_buffer=state_buffer)
+                                      a0.Nrefine, a0.update_method, device=self.device, state_buffer=state_buffer,
+                                      ensemble=mbd_mpc.plan_ensemble(self.args))
         e.load_schedule(colds)   # sigma = 1.0 in every row (path_integral.py:140)
         return e
 

@@ -8,7 +8,8 @@ run_pi_mpc_batch) at the same Nsample, Hsample, Nwarm and Nstep, the cold solve 
 planner's recommended temperature for the env.  `zero` is the plant under zero actions from the same reset states.  Per algorithm
 one line: the closed-loop mean reward over the seeds and the wall time of one warm control step of the whole batch.
 `--plant_friction` / `--plant_gear` run every algorithm and the zero-action baseline against a plant whose contact friction and
-actuator gear are scaled by those factors, while the planners keep the nominal model (DESIGN.md §5k).
+actuator gear are scaled by those factors, while the planners keep the nominal model (DESIGN.md §5k).  `--plan_friction` /
+`--plan_gear` (K values each) let every algorithm plan against the ensemble of the K models (DESIGN.md §5l).
 """
 from __future__ import annotations
 
@@ -35,13 +36,16 @@ class Args:
     sigma_warm: float = 1.0  # the baselines' sampling sigma at the start of every warm control step
     plant_friction: float = 1.0  # the plant's contact friction over the planners' model (xpbd envs)
     plant_gear: float = 1.0  # the plant's actuator gear over the planners' model (xpbd envs)
+    plan_friction: tuple[float, ...] = ()  # the planners' ensemble: member k's friction factor (xpbd envs; empty = nominal)
+    plan_gear: tuple[float, ...] = ()  # member k's actuator-gear factor (as many as plan_friction)
 
 
 def mbd_args(args: Args, seeds=SEEDS):
     temp = mbd_planner.TEMP_RECOMMEND.get(args.env_name, mbd_planner.Args.temp_sample)
     return [mbd_mpc.Args(seed=s, env_name=args.env_name, Nsample=args.Nsample, Hsample=args.Hsample, Ndiffuse=args.Nsolve,
                          Nwarm=args.Nwarm, Nstep=args.Nstep, temp_sample=temp, plant_friction=args.plant_friction,
-                         plant_gear=args.plant_gear, not_render=True, disable_recommended_params=True)
+                         plant_gear=args.plant_gear, plan_friction=tuple(args.plan_friction), plan_gear=tuple(args.plan_gear),
+                         not_render=True, disable_recommended_params=True)
             for s in seeds]
 
 
@@ -49,8 +53,8 @@ def pi_args(args: Args, method: str, seeds=SEEDS):
     temp = path_integral.TEMP_RECOMMEND.get(args.env_name, path_integral.Args.temp_sample)
     return [pi_mpc.Args(seed=s, env_name=args.env_name, update_method=method, Nsample=args.Nsample, Hsample=args.Hsample,
                         Nrefine=args.Nsolve, Nwarm=args.Nwarm, Nstep=args.Nstep, sigma_warm=args.sigma_warm, temp_sample=temp,
-                        plant_friction=args.plant_friction, plant_gear=args.plant_gear, not_render=True,
-                        disable_recommended_params=True) for s in seeds]
+                        plant_friction=args.plant_friction, plant_gear=args.plant_gear, plan_friction=tuple(args.plan_friction),
+                        plan_gear=tuple(args.plan_gear), not_render=True, disable_recommended_params=True) for s in seeds]
 
 
 def zero_action_rewards(env, states0: np.ndarray, Nstep: int, friction=1.0, gear=1.0) -> np.ndarray:
