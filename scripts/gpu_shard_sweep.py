@@ -1,5 +1,5 @@
 """Shard-size sweep of the rollout kernels: every kernel variant at the per-GPU shard sizes of a strong-scaling run
-(8192 samples over 8 / 4 / 2 / 1 GPUs) — the data behind the auto-selector in launch_rollout (csrc/mbd_b200.cu).
+(8192 samples over 8 / 4 / 2 / 1 GPUs) — the data behind the auto-selector in choose_kernel (csrc/mbd_b200.cu).
 Each variant is checked bit for bit against variant 2.  --lib loads another build of the library (e.g. an older commit's
 libmbd_b200.so) instead of the tree's, so that two builds can be timed in alternating runs on one GPU.
     python scripts/gpu_shard_sweep.py [env] [out.json] [--lib PATH]"""

@@ -7,7 +7,7 @@ the oracle:
 * `k_car2d` from x0 and family starts and from undecided rim states, and `k_car2d_ps` on every constructed one-step family: an undecided step equals the
   frozen state bit for bit or lies within K radii of q_new;
 * `k_pusht` on every pushT family at mu = 1 and 0 in both solver modes: within K radii of one enumerated configuration.
-The per-env-state kernels `k_rollout_ps`, `k_rollout_wpl_ps` and `k_pusht_ps` step a whole env step; they equal the broadcast
+The per-env-state kernels `k_rollout<PerEnv>`, `k_rollout_wpl<PerEnv>` and `k_pusht_ps` step a whole env step; they equal the broadcast
 kernels above bit for bit from the same state (tests/test_horizon_f64_gpu.py), so these checks hold them too."""
 import numpy as np
 import pytest

@@ -9,7 +9,7 @@ selector picks the kernel itself:
 * that the loop carries nothing but the 13 words per link: a relaunch from a substep's or an env step's state (n = 1)
   gives the next one bit for bit, and the relaunched substeps along the horizon stay within the bound;
 * the fused sampling kernels, whose returns equal `ops.rollout` on the actions they drew, so the checks above cover them;
-* the vector env's per-env-state kernels (`k_rollout_ps`, `k_rollout_wpl_ps`, `k_pusht_ps`): one family state per env,
+* the vector env's per-env-state kernels (`k_rollout<PerEnv>`, `k_rollout_wpl<PerEnv>`, `k_pusht_ps`): one family state per env,
   next state and reward bit for bit against the broadcast kernel from that state, reward within the float64 bound."""
 import hashlib
 
@@ -56,7 +56,7 @@ def big_n():
 
 def ps_kernel(blob, nenv):
     """the kernel `mbd_vec_step` (csrc/mbd_b200.cu) runs for an xpbd vector env of nenv envs"""
-    return "k_rollout_ps" if int(blob.view(np.int32)[B.H_NLINK]) == 11 and nenv <= 16 * sms() else "k_rollout_wpl_ps"
+    return "k_rollout<PerEnv>" if int(blob.view(np.int32)[B.H_NLINK]) == 11 and nenv <= 16 * sms() else "k_rollout_wpl<PerEnv>"
 
 
 VEC_CASES = [(m, 67) for m in F.SHIPPED + ["contact_params", "gen3"]] + [(m, "big") for m in HUMANOIDS + ["gen100"]]
@@ -68,7 +68,7 @@ def test_every_kernel_is_covered(tmp_path):
     got |= {launched_kernel(F.make_env(m, tmp_path).blob, 0, big_n(), sms()) for m in HUMANOIDS}
     got |= {ps_kernel(F.make_env(m, tmp_path).blob, big_n() if nb == "big" else nb) for m, nb in VEC_CASES}
     got.add("k_pusht_ps")      # test_vecenv_pusht_step_within_the_float64_bound: the only kernel of the pushT vector env
-    want = {"lane-per-link", "wpl-cta", "wpl-named", "wpl-generic", "pk-group", "k_rollout_ps", "k_rollout_wpl_ps", "k_pusht_ps"}
+    want = {"lane-per-link", "wpl-cta", "wpl-named", "wpl-generic", "pk-group", "k_rollout<PerEnv>", "k_rollout_wpl<PerEnv>", "k_pusht_ps"}
     assert want <= got, want - got
 
 
@@ -235,7 +235,7 @@ def _family_states(env, name):
 
 @pytest.mark.parametrize("name,nenv", VEC_CASES)
 def test_vecenv_step_within_the_float64_bound(tmp_path, name, nenv):
-    """k_rollout_ps / k_rollout_wpl_ps: env b starts at family state b mod S with its own action.  Its next state and reward
+    """k_rollout<PerEnv> / k_rollout_wpl<PerEnv>: env b starts at family state b mod S with its own action.  Its next state and reward
     equal ops.rollout from that state bit for bit; its reward is within the float64 bound of its own two states."""
     env = F.make_env(name, tmp_path)
     nenv = big_n() if nenv == "big" else nenv

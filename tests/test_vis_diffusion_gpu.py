@@ -1,4 +1,4 @@
-"""The recorded rollout (`ops.rollout(..., want_traj=True)`, k_rollout_wpl_traj) and the diffusion-process page on the device:
+"""The recorded rollout (`ops.rollout(..., want_traj=True)`, k_rollout_wpl<Traj>) and the diffusion-process page on the device:
 every recorded state against H successive one-step `ops.rollout` calls, bit for bit, on the shipped humanoids, hopper, ant and a
 random model, at one sample, 77 and more than 16 per SM (which crosses every kernel the selector picks for the plain rollout); the
 other outputs against the rollout without a record; the world poses of every iterate against host `env.step`; pushT; and the

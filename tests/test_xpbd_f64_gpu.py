@@ -19,7 +19,7 @@ CASES = [(m, v) for m in HUMANOIDS for v in (0, 1, 2, 3, 8)] + [(m, v) for m in 
 
 
 def launched_kernel(blob, variant, n, sms):
-    """the rollout kernel `launch_rollout` (csrc/mbd_b200.cu) runs for a requested variant: it remaps variants a model cannot
+    """the rollout kernel `choose_kernel` (csrc/mbd_b200.cu) runs for a requested variant: it remaps variants a model cannot
     take (named barriers need 2 per parent within 15, the packed kernel 11 hinge-only links with at most 2 contacts each)"""
     bi = blob.view(np.int32)
     L = int(bi[B.H_NLINK])
