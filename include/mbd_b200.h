@@ -200,15 +200,39 @@ typedef struct mbd_step_plan {
   /* planner ensemble (appended; mbd_batch_step_launch / mbd_pi_batch_step_launch only, xpbd envs, DESIGN.md §5l).  Problem b
    * rolls every sample Y_bn out under ens_k models (f_bk, g_bk): every contact friction fl(mu * f_bk), every actuator gear
    * fl(gear * g_bk).  ens_rews[b][n][k] receives each member return r_bnk; the sample return the tail reads is
-   * rews[b][n] = fl(fl(fl(r_bn0 + r_bn1) + ...) / ens_k), summed in member order.  NULL / 0 = today's step. */
+   * rews[b][n] = fl(fl(fl(r_bn0 + r_bn1) + ...) / ens_k), summed in member order.  NULL / 0 = today's step.
+   * ens_worst = m >= 1 scores a sample by its m worst members instead (DESIGN.md §5m): NaN (0x7fffffff) if any r_bnk is NaN,
+   * otherwise the K returns sorted ascending, ties by member index, s = r_(0), s = fl(s + r_(j)) for j = 1 .. m - 1, and
+   * rews[b][n] = fl(s / m).  m = 1 is the minimum, m = K / 2 a discrete CVaR at 50 %.  0 = the ordered mean above. */
   const float* ens_factors_dev;      /* [B][ens_k][2]: friction factor, gear factor of every member of every problem */
   float* ens_rews_dev;               /* [B][N][ens_k] */
   int32_t ens_k;                     /* members per problem, 1 .. MBD_ENS_MAXK with a table, 0 without */
-  int32_t ens_pad;
+  int32_t ens_worst;                 /* 0 .. ens_k with a table (0 = the mean), 0 without */
 } mbd_step_plan;
 #define MBD_ENS_MAXK 16
 /* sizeof(mbd_step_plan), offsetof ens_factors_dev / ens_rews_dev / ens_k and MBD_ENS_MAXK (cross-checked against the ctypes mirror) */
 int mbd_ens_abi_sizes(int32_t* out, int n);
+/* sizeof(mbd_step_plan), offsetof ens_worst, sizeof(mbd_ens_draw_plan) and offsetof its keys_dev / ranges_dev / mpc_ctl_dev /
+ * ens_factors_dev (cross-checked against the ctypes mirror) */
+int mbd_ens_risk_abi_sizes(int32_t* out, int n);
+/* Test entry point: the score launch of an ensemble step alone, on whatever the caller put into ens_rews_dev [count][K]:
+ * rews_dev [count] <- the ordered mean (worst == 0) or the worst-m score (m = worst) of each row.  MBD_EINVAL before any CUDA call for a
+ * NULL buffer, count < 1, K outside 1 .. MBD_ENS_MAXK or worst outside 0 .. K. */
+int mbd_ens_score(const float* ens_rews_dev, float* rews_dev, int count, int K, int worst, mbd_stream s);
+/* Members drawn afresh at every control step of the receding-horizon controllers (DESIGN.md §5m).  One launch, one thread per
+ * (problem b, member k), graph-capturable: with c = mpc_ctl[b] and c < Nstep, (kf, kg) = split(keys[b][c]) and
+ * ens_factors[b][k] = (uniform(kf, (K,), flo_b, fhi_b)[k], uniform(kg, (K,), glo_b, ghi_b)[k]) in the threefry layout of the
+ * samplers (prng.split / prng.uniform); a problem with c outside 0 .. Nstep - 1 is not written.  MBD_EINVAL before any CUDA call
+ * for a NULL plan or buffer, B outside 1 .. MBD_VEC_MAX_B, K outside 1 .. MBD_ENS_MAXK or Nstep < 1.  The ranges are the caller's
+ * to check (finite, 0 <= lo <= hi). */
+typedef struct mbd_ens_draw_plan {
+  int32_t B, K, Nstep, pad;
+  const uint32_t* keys_dev;          /* [B][Nstep][2]: the member key of every control step of every problem */
+  const float* ranges_dev;           /* [B][4]: friction lo, friction hi, gear lo, gear hi */
+  const int32_t* mpc_ctl_dev;        /* [B]: the control step counter of mbd_mpc_advance */
+  float* ens_factors_dev;            /* [B][K][2]: mbd_step_plan.ens_factors_dev */
+} mbd_ens_draw_plan;
+int mbd_ens_draw(const mbd_ens_draw_plan* plan, mbd_stream s);
 /* mbd_step_launch, mbd_step_launch_ev and mbd_step_tail_launch refuse an ensemble (MBD_EINVAL): the single-solve, sharded and
  * benchmark step keep their three launches. */
 int mbd_step_launch(const mbd_step_plan* plan, mbd_stream s);

@@ -42,7 +42,7 @@ class StepPlan(ctypes.Structure):
         ("peer_base_ptrs", ctypes.POINTER(ctypes.c_uint64)),
         ("off_rews_words", ctypes.c_uint64), ("off_logpd_words", ctypes.c_uint64), ("off_partial_words", ctypes.c_uint64),
         ("off_flags_words", ctypes.c_uint64), ("timeout_cycles", ctypes.c_uint64),
-        ("ens_factors_dev", c_vp), ("ens_rews_dev", c_vp), ("ens_k", ctypes.c_int32), ("ens_pad", ctypes.c_int32),
+        ("ens_factors_dev", c_vp), ("ens_rews_dev", c_vp), ("ens_k", ctypes.c_int32), ("ens_worst", ctypes.c_int32),
     ]
 
 
@@ -121,6 +121,12 @@ class MpcPiPlan(ctypes.Structure):
     _fields_ = [("base", MpcPlan), ("sigma_warm", ctypes.c_float), ("pad", ctypes.c_int32), ("sigma_log_dev", c_vp)]
 
 
+class EnsDrawPlan(ctypes.Structure):
+    """mbd_ens_draw_plan (include/mbd_b200.h): the planner ensemble drawn afresh at every control step"""
+    _fields_ = [("B", ctypes.c_int32), ("K", ctypes.c_int32), ("Nstep", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("keys_dev", c_vp), ("ranges_dev", c_vp), ("mpc_ctl_dev", c_vp), ("ens_factors_dev", c_vp)]
+
+
 MPC_ACT, MPC_RECORD = 0, 1                                     # MBD_MPC_*
 PPO_ACT, PPO_RECORD, PPO_EVAL, PPO_EVAL_RECORD = 0, 1, 2, 3   # MBD_PPO_*
 PPO_MAX_OBS, PPO_MAX_NU, PPO_MAX_MB, PPO_STAT_ROWS = 128, 32, 4096, 256
@@ -196,6 +202,9 @@ def lib():
                                            ctypes.POINTER(PiBufs), ctypes.c_int, c_vp]
     L.mbd_pi_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_ens_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_ens_risk_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
+    L.mbd_ens_score.argtypes = [c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp]
+    L.mbd_ens_draw.argtypes = [ctypes.POINTER(EnsDrawPlan), c_vp]
     L.mbd_bbo_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
                                             ctypes.POINTER(BboBufs), c_vp]
     L.mbd_bbo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
@@ -239,7 +248,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_ens_abi_sizes", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_ens_abi_sizes", "mbd_ens_risk_abi_sizes", "mbd_ens_score", "mbd_ens_draw", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
 
 

@@ -68,4 +68,23 @@ __global__ void __launch_bounds__(kMpcThreads) k_mpc_advance(mbd_mpc_plan p, int
   }
 }
 
+// k_ens_draw (mbd_ens_draw): the planner ensemble of control step c = mpc_ctl[b], one thread per (problem b, member k).  It runs
+// before the control step's diffusion steps, so c is the step about to be planned; past the last control step it writes nothing.
+constexpr int kEnsDrawThreads = 128;
+
+__global__ void __launch_bounds__(kEnsDrawThreads) k_ens_draw(mbd_ens_draw_plan p, int part) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= p.B * p.K) return;
+  const int b = t / p.K, k = t - b * p.K;
+  const int c = p.mpc_ctl_dev[b];
+  if (c < 0 || c >= p.Nstep) return;
+  const uint32_t* key = p.keys_dev + ((size_t)b * p.Nstep + c) * 2;
+  const float* R = p.ranges_dev + (size_t)b * 4;
+  uint32_t kf[2], kg[2];
+  vec_split(key[0], key[1], 2, 0, part, kf);
+  vec_split(key[0], key[1], 2, 1, part, kg);
+  p.ens_factors_dev[(size_t)t * 2] = vec_uniform(kf, k, p.K, part, R[0], R[1]);
+  p.ens_factors_dev[(size_t)t * 2 + 1] = vec_uniform(kg, k, p.K, part, R[2], R[3]);
+}
+
 }  // namespace mbd

@@ -312,6 +312,21 @@ def mpc_pi_advance(plan: "_lib.MpcPiPlan", mode: int):
     check(_lib.lib().mbd_mpc_pi_advance(ctypes.byref(plan), int(mode), _stream()), "mbd_mpc_pi_advance")
 
 
+def ens_draw(plan: "_lib.EnsDrawPlan"):
+    """the planner ensemble of every problem's current control step, drawn on the device (mbd_ens_draw, DESIGN.md §5m)"""
+    check(_lib.lib().mbd_ens_draw(ctypes.byref(plan), _stream()), "mbd_ens_draw")
+
+
+def ens_score(ens_rews: torch.Tensor, worst: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """the score launch of an ensemble step alone (mbd_ens_score): ens_rews [..., K] member returns -> [...] sample returns, the
+    ordered mean (worst = 0) or the worst-m score (m = worst); the entry point the score tests drive with constructed returns"""
+    ens_rews = _dev(ens_rews)
+    K = ens_rews.shape[-1]
+    out = torch.empty(ens_rews.shape[:-1], device=ens_rews.device, dtype=torch.float32) if out is None else _dev(out)
+    check(_lib.lib().mbd_ens_score(_p(ens_rews), _p(out), int(out.numel()), int(K), int(worst), _stream()), "mbd_ens_score")
+    return out
+
+
 def step_tail_launch(plan: "_lib.StepPlan"):
     """launches 2 and 3 of a step only (statistics + softmax, weighted mean + update) on the inputs already in the plan's
     buffers: mbd_step_tail_launch, the entry point the tail tests drive with constructed returns and samples"""

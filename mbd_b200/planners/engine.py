@@ -124,6 +124,18 @@ def ensemble_table(table, B: int, env, enable_demo: bool) -> np.ndarray:
     return f
 
 
+def check_ens_worst(worst, K: Optional[int]) -> int:
+    """mbd_step_plan.ens_worst of an ensemble of K members (None: no ensemble): an int in 0 .. K, and 0 without an ensemble
+    (ValueError)"""
+    if isinstance(worst, bool) or not isinstance(worst, (int, np.integer)):
+        raise ValueError(f"ens_worst must be an int (got {worst!r})")
+    if K is None and worst != 0:
+        raise ValueError(f"ens_worst = {worst} needs a planner ensemble")
+    if K is not None and not 0 <= worst <= K:
+        raise ValueError(f"ens_worst must be in 0 .. K = {K} (got {worst})")
+    return int(worst)
+
+
 def xref_len(env, xref) -> int:
     """href of the step plan: the demonstration's length in steps (0 without one)"""
     return 0 if xref is None else int(xref.shape[1] if env.kind == "xpbd" else xref.shape[0])
@@ -348,18 +360,23 @@ class BatchedDiffusionEngine:
 
     ensemble: a planner ensemble [B][K][2] (DESIGN.md §5l, positional envs, no demo): problem b rolls every sample out under the K
     models (friction ensemble[b][k][0], gear ensemble[b][k][1]) and the tail reads the mean of the K returns.  `ens_rews` [B, N, K]
-    holds every member return of the last step.  None: today's step."""
+    holds every member return of the last step.  None: today's step.
+
+    ens_worst: with an ensemble, m in 1 .. K scores every sample by the mean of its m worst member returns instead of all K
+    (DESIGN.md §5m; 1 = the minimum).  0: the mean.  A captured step bakes it in, so it is fixed at construction."""
 
     ens_factors: Optional[torch.Tensor] = None   # [B, K, 2] on the device once an ensemble is given
     ens_rews: Optional[torch.Tensor] = None      # [B, N, K]
 
     def __init__(self, env, Nsample: int, Hsample: int, temps, enable_demo: bool, state_inits, Ndiffuse: int,
-                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None):
+                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None,
+                 ens_worst: int = 0):
         self.env = env
         self.B = len(state_inits)
         if self.B < 1 or len(temps) != self.B:
             raise ValueError(f"{self.B} initial states and {len(temps)} temperatures: need one of each per problem, B >= 1")
         ens = None if ensemble is None else ensemble_table(ensemble, self.B, env, enable_demo)
+        self.ens_worst = check_ens_worst(ens_worst, None if ens is None else ens.shape[1])
         self.N, self.H = int(Nsample), int(Hsample)
         self.enable_demo = bool(enable_demo)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -386,6 +403,7 @@ class BatchedDiffusionEngine:
             self.ens_rews = torch.empty((self.B, self.N, K), device=self.device, dtype=torch.float32)
             p = self._plan_c
             p.ens_factors_dev, p.ens_rews_dev, p.ens_k = self.ens_factors.data_ptr(), self.ens_rews.data_ptr(), K
+            p.ens_worst = self.ens_worst
 
     def set_ensemble(self, table):
         """rewrites the planner ensemble in place (same B and K): a captured step reads the new values on its next replay"""

@@ -10,11 +10,14 @@ Nwarm ... 1 on the same schedule rows as the Ndiffuse-step solve, with the keys 
 The plant may differ from the model the planner plans with (DESIGN.md §5k): `plant_friction` and `plant_gear` scale every contact
 friction and every actuator gear of the plant of one problem (`envs.vec.scaled_env`), while the planner keeps the nominal model.
 The planner may plan against an ensemble of models instead (DESIGN.md §5l): with `plan_friction` / `plan_gear` of length K every
-sample is rolled out under the K models (plan_friction[k], plan_gear[k]) and scored by the mean of the K returns.
+sample is rolled out under the K models (plan_friction[k], plan_gear[k]) and scored by the mean of the K returns.  With
+`plan_members = K` the K members are drawn afresh at every control step from `plan_friction_range` x `plan_gear_range` with a key
+chain of the problem's own (DESIGN.md §5m, `member_keys`), and `plan_worst = m >= 1` scores a sample by the mean of its m worst
+member returns instead of all K (1 = the minimum).
 
 Everything runs on the device: B closed loops (one per seed) share one `BatchedDiffusionEngine` that plans from the state buffer of
-a `VecEnv`, and `mbd_mpc_advance` executes the plan and re-arms the next control step.  A warm control step (Nwarm batched
-diffusion steps, ACT, the env step, RECORD) is one captured CUDA graph:
+a `VecEnv`, and `mbd_mpc_advance` executes the plan and re-arms the next control step.  A warm control step (the member draw when
+members are drawn, Nwarm batched diffusion steps, ACT, the env step, RECORD) is one captured CUDA graph:
 
     python -m mbd_b200.planners.mbd_mpc --env_name hopper --Nwarm 10 --Nstep 50
 """
@@ -54,6 +57,13 @@ class Args(mbd_planner.Args):
     # for every problem of a batch, values per problem); empty = the nominal model
     plan_friction: tuple[float, ...] = ()
     plan_gear: tuple[float, ...] = ()
+    # drawn planner ensemble: plan_members = K members drawn afresh at every control step, friction uniform in plan_friction_range
+    # and gear uniform in plan_gear_range ((lo, hi) with 0 <= lo <= hi, per problem); 0 = none.  Excludes plan_friction / plan_gear
+    plan_members: int = 0
+    plan_friction_range: tuple[float, ...] = ()
+    plan_gear_range: tuple[float, ...] = ()
+    # risk measure of either ensemble: score a sample by the mean of its plan_worst worst member returns (1 .. K); 0 = the mean
+    plan_worst: int = 0
 
 
 # fields every problem of one run_mpc_batch call must share; seed, temp_sample, beta0 and betaT may differ
@@ -97,33 +107,86 @@ def check_plant(args_list) -> None:
 
 
 def check_plan(args_list) -> None:
-    """plan_friction / plan_gear: equal lengths K <= ENS_MAXK, the same K for every problem, values finite and >= 0, and empty on
-    car2d and pushT (ValueError)"""
-    ks = set()
+    """plan_friction / plan_gear: equal lengths K <= ENS_MAXK, values finite and >= 0.  plan_members: 0 .. ENS_MAXK, not together
+    with plan_friction / plan_gear, with both ranges (lo, hi) finite in float32 and 0 <= lo <= hi, and a seed in 0 .. 2^32 - 1;
+    ranges without plan_members are refused.  plan_worst: 0 .. K, 0 without an ensemble.  K, plan_worst and whether members are
+    drawn are the same for every problem; car2d and pushT plan with the nominal model (ValueError)"""
+    ks, worsts, drawn = set(), set(), set()
     for a in args_list:
         fr, gr = tuple(a.plan_friction), tuple(a.plan_gear)
         if len(fr) != len(gr):
             raise ValueError(f"plan_friction and plan_gear must have the same length (got {len(fr)} and {len(gr)})")
         if len(fr) > _lib.ENS_MAXK:
             raise ValueError(f"a planner ensemble has at most {_lib.ENS_MAXK} members (got {len(fr)})")
-        if fr and a.env_name in ("car2d", "pushT"):
-            raise ValueError(f"planner ensembles exist for the positional (xpbd) envs only, not {a.env_name}")
         for f, vals in (("plan_friction", fr), ("plan_gear", gr)):
             with np.errstate(over="ignore"):
                 v32 = np.asarray(vals, dtype=np.float64).astype(np.float32)
             if not (np.isfinite(v32).all() and (v32 >= 0).all()):
                 raise ValueError(f"{f} must be finite and >= 0 in float32 (got {vals})")
-        ks.add(len(fr))
+        M = a.plan_members
+        if isinstance(M, bool) or not isinstance(M, (int, np.integer)) or not 0 <= M <= _lib.ENS_MAXK:
+            raise ValueError(f"plan_members must be an int in 0 .. {_lib.ENS_MAXK} (got {M!r})")
+        if M and fr:
+            raise ValueError("plan_members draws the ensemble: it excludes plan_friction / plan_gear")
+        for f in ("plan_friction_range", "plan_gear_range"):
+            rng = tuple(getattr(a, f))
+            if not M:
+                if rng:
+                    raise ValueError(f"{f} needs plan_members >= 1 (the members it draws)")
+                continue
+            if len(rng) != 2:
+                raise ValueError(f"{f} must be (lo, hi) when plan_members >= 1 (got {rng})")
+            with np.errstate(over="ignore"):
+                lo, hi = (float(np.float32(v)) for v in rng)
+            if not (math.isfinite(lo) and math.isfinite(hi) and 0 <= lo <= hi):
+                raise ValueError(f"{f} must be (lo, hi) with 0 <= lo <= hi, finite in float32 (got {rng})")
+        if M and not 0 <= a.seed < 1 << 32:
+            raise ValueError(f"drawn members need a seed in 0 .. 2^32 - 1 (got {a.seed})")
+        K = M or len(fr)
+        if K and a.env_name in ("car2d", "pushT"):
+            raise ValueError(f"planner ensembles exist for the positional (xpbd) envs only, not {a.env_name}")
+        w = a.plan_worst
+        if isinstance(w, bool) or not isinstance(w, (int, np.integer)):
+            raise ValueError(f"plan_worst must be an int (got {w!r})")
+        if w and not K:
+            raise ValueError(f"plan_worst = {w} needs a planner ensemble (plan_friction / plan_gear or plan_members)")
+        if not 0 <= w <= K:
+            raise ValueError(f"plan_worst must be in 0 .. K = {K} (got {w})")
+        ks.add(K)
+        worsts.add(int(w))
+        drawn.add(bool(M))
     if len(ks) > 1:
         raise ValueError(f"every problem of a batch must plan with the same number of ensemble members (got {sorted(ks)})")
+    if len(drawn) > 1:
+        raise ValueError("every problem of a batch must draw its members (plan_members) or none may")
+    if len(worsts) > 1:
+        raise ValueError(f"every problem of a batch must plan with the same plan_worst (got {sorted(worsts)})")
 
 
 def plan_ensemble(args_list):
     """the [B, K, 2] planner ensemble of the problems (member k of problem b = (plan_friction[k], plan_gear[k])), or None when
-    they plan with the nominal model"""
+    they plan with the nominal model.  Drawn members start as the ones of (1, 1): the draw of control step 0 replaces them before
+    the first diffusion step."""
+    if args_list[0].plan_members:
+        return np.ones((len(args_list), args_list[0].plan_members, 2), np.float32)
     if not args_list[0].plan_friction:
         return None
     return np.array([[(f, g) for f, g in zip(a.plan_friction, a.plan_gear)] for a in args_list], dtype=np.float32)
+
+
+def member_keys(seed: int, Nstep: int) -> np.ndarray:
+    """[Nstep, 2] the member key of every control step of the loop of `seed` (0 <= seed < 2^32): split(PRNGKey(2^32 | seed), Nstep).
+    The root key [1, seed] differs from the controller's [0, seed] (mpc_keys), so the two chains share no key."""
+    return prng.split(prng.PRNGKey((1 << 32) | int(seed)), Nstep)
+
+
+def draw_members(key, K: int, friction_range, gear_range) -> np.ndarray:
+    """[K, 2] the members drawn with one control step's member key: kf, kg = split(key); member k = (uniform(kf, (K,), flo, fhi)[k],
+    uniform(kg, (K,), glo, ghi)[k]).  The specification of mbd_ens_draw."""
+    kf, kg = prng.split(key)
+    f = prng.uniform(kf, (K,), friction_range[0], friction_range[1])
+    g = prng.uniform(kg, (K,), gear_range[0], gear_range[1])
+    return np.stack([f, g], axis=1).astype(np.float32)
 
 
 def plant_factors(args_list):
@@ -219,6 +282,21 @@ class Controller:
         self.rewards = torch.zeros((self.B, self.Nstep), **f)
         self.states = torch.zeros((self.B, self.Nstep + 1, self.S), **f)
         self.rew_hist = torch.zeros((self.B, self.Nstep), **f)
+        self.draws = None      # [B, Nstep, K, 2] the host's drawn members (host-driven loop)
+        self.draw_plan = None  # mbd_ens_draw's plan (device loop)
+        if a0.plan_members:
+            mk = np.stack([member_keys(a.seed, self.Nstep) for a in args_list])                  # [B, Nstep, 2] uint32
+            ranges = np.array([tuple(a.plan_friction_range) + tuple(a.plan_gear_range) for a in args_list], np.float32)
+            if self.host:
+                self.draws = np.stack([np.stack([draw_members(mk[b, c], a0.plan_members, ranges[b, :2], ranges[b, 2:])
+                                                 for c in range(self.Nstep)]) for b in range(self.B)])
+            else:
+                self.member_keys = torch.as_tensor(mk.view(np.int32), device=d).contiguous()
+                self.ranges = torch.as_tensor(ranges, device=d).contiguous()
+                dp = self.draw_plan = _lib.EnsDrawPlan()
+                dp.B, dp.K, dp.Nstep = self.B, a0.plan_members, self.Nstep
+                dp.keys_dev, dp.ranges_dev = self.member_keys.data_ptr(), self.ranges.data_ptr()
+                dp.mpc_ctl_dev, dp.ens_factors_dev = self.mpc_ctl.data_ptr(), self.engine.ens_factors.data_ptr()
         self.graph = None
         self.warm_seconds = 0.0    # wall time of control steps 1 ... Nstep - 1 of the last run (synchronised at both ends)
         self.plan = self._make_plan() if not self.host else None
@@ -231,7 +309,8 @@ class Controller:
             print(f"init sigma = {sigmas[-1]:.2e}")
             scheds.append((sigmas, alphas, alphas_bar))
         e = BatchedDiffusionEngine(self.env, a0.Nsample, a0.Hsample, [a.temp_sample for a in self.args], False, self.host_states,
-                                   a0.Ndiffuse, device=self.device, state_buffer=state_buffer, ensemble=plan_ensemble(self.args))
+                                   a0.Ndiffuse, device=self.device, state_buffer=state_buffer, ensemble=plan_ensemble(self.args),
+                                   ens_worst=a0.plan_worst)
         e.load_schedule(colds, [s[0] for s in scheds], [s[1] for s in scheds], [s[2] for s in scheds])
         return e
 
@@ -263,7 +342,13 @@ class Controller:
     def _host_sigma(self, c: int, more: bool):
         """the host-driven loop's share of what ACT does to the sampling sigmas at control step c (nothing for this planner)"""
 
+    def _draw(self):
+        """the members of every problem's current control step (mbd_ens_draw), when members are drawn"""
+        if self.draw_plan is not None:
+            ops.ens_draw(self.draw_plan)
+
     def _warm_step(self):
+        self._draw()
         for _ in range(self.Nwarm):
             self.engine._launch()
         self._execute()
@@ -282,6 +367,7 @@ class Controller:
         graph = os.environ.get("MBD_GRAPH", "1") != "0" if graph is None else graph
         e = self.engine
         with torch.cuda.device(self.device):
+            self._draw()                        # control step 0's members, before the cold solve
             if graph:
                 e.capture()
             for _ in range(self.Nd - 1):        # control step 0: run_diffusion's solve
@@ -316,7 +402,8 @@ class Controller:
     # ---- the host-driven loop ---------------------------------------------------------------------------------------------
     def run_host_driven(self) -> MpcResult:
         """the same arithmetic with the host in the loop: eager batched steps, then per control step the plan is copied to the
-        host, every plant is stepped by the host `env.step`, and the warm start, keys and step counters are written with torch"""
+        host, every plant is stepped by the host `env.step`, and the warm start, keys and step counters are written with torch.  Drawn
+        members are drawn on the host (`draw_members`) and written with `set_ensemble` before each control step's diffusion steps"""
         if not self.host:
             raise ValueError("this controller was built for the device loop")
         e, B, Nu, nw, env = self.engine, self.B, self.Nu, self.Nwarm, self.env
@@ -331,6 +418,8 @@ class Controller:
                 if c == 1:
                     torch.cuda.synchronize()
                     t0 = time.perf_counter()
+                if self.draws is not None:
+                    e.set_ensemble(self.draws[:, c])
                 for _ in range(self.Nd - 1 if c == 0 else nw):
                     e.step()
                 P = e.Ybars[:, 0].reshape(B, self.H, Nu)

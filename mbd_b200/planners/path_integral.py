@@ -137,14 +137,15 @@ class BatchedPathIntegralEngine(BatchedDiffusionEngine):
     capture, check_exchange, problem).  Ybars[b] holds problem b's means: row t = mu_0t of step t, row t-1 its result; launch (1)
     reads sigma_t from params[b][t].sigma.  CMA-ES writes sigma' to params[b][t-1].sigma and sigma_hist[b][t-1] on the device.
     Problem b draws the noise of a stand-alone solve with its own key and reduces in the same order, so it reproduces the B = 1
-    solve of the same inputs bit for bit.  state_buffer and ensemble: as in BatchedDiffusionEngine (the receding-horizon controller
+    solve of the same inputs bit for bit.  state_buffer, ensemble and ens_worst: as in BatchedDiffusionEngine (the receding-horizon controller
     of pi_mpc.py passes `VecEnv.state`)."""
 
     def __init__(self, env, Nsample: int, Hsample: int, temps, state_inits, Nrefine: int, update_method: str,
-                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None):
+                 device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None,
+                 ens_worst: int = 0):
         if update_method not in _lib.PI_METHODS:
             raise KeyError(update_method)
-        super().__init__(env, Nsample, Hsample, temps, False, state_inits, Nrefine, device, state_buffer, ensemble)
+        super().__init__(env, Nsample, Hsample, temps, False, state_inits, Nrefine, device, state_buffer, ensemble, ens_worst)
         self.update_method = update_method
         self.method = _lib.PI_METHODS[update_method]
         d, f = self.device, dict(device=self.device, dtype=torch.float32)

@@ -11,7 +11,8 @@ The sampling sigma is **reset, not carried**: every control step c >= 1 starts f
 adapts it inside the control step as the reference's update does, and the sigma each control step ends with is logged
 (`MpcResult.sigmas`).  A carried CMA-ES sigma would sit at the reference's 1e-3 floor after the first solve and could not re-plan.
 With `sigma_warm = 1.0` a warm step is the reference's update verbatim.  `plant_friction` / `plant_gear` give every problem its
-own plant and `plan_friction` / `plan_gear` a planner ensemble, as in mbd_mpc.py.
+own plant, `plan_friction` / `plan_gear` a planner ensemble, `plan_members` with its two ranges members drawn at every control step
+and `plan_worst` a worst-m score, as in mbd_mpc.py.
 
 Everything runs on the device: the B loops share one `BatchedPathIntegralEngine` that plans from the state buffer of a `VecEnv`,
 `mbd_mpc_pi_advance` executes the plan, re-arms the next control step and resets its sigma rows, and a warm control step (Nwarm
@@ -47,6 +48,12 @@ class Args(path_integral.Args):
     # planner ensemble (mbd_mpc.Args): member k plans with (plan_friction[k], plan_gear[k]); empty = the nominal model
     plan_friction: tuple[float, ...] = ()
     plan_gear: tuple[float, ...] = ()
+    # drawn planner ensemble and its risk measure (mbd_mpc.Args): K = plan_members members drawn at every control step from the
+    # two (lo, hi) ranges; plan_worst = m scores a sample by its m worst members (0 = the mean)
+    plan_members: int = 0
+    plan_friction_range: tuple[float, ...] = ()
+    plan_gear_range: tuple[float, ...] = ()
+    plan_worst: int = 0
 
 
 # fields every problem of one run_pi_mpc_batch call must share; seed and temp_sample may differ
@@ -95,7 +102,7 @@ class Controller(mbd_mpc.Controller):
         self.sigmas = torch.zeros((self.B, self.Nstep), device=self.device, dtype=torch.float32)
         e = BatchedPathIntegralEngine(self.env, a0.Nsample, a0.Hsample, [a.temp_sample for a in self.args], self.host_states,
                                       a0.Nrefine, a0.update_method, device=self.device, state_buffer=state_buffer,
-                                      ensemble=mbd_mpc.plan_ensemble(self.args))
+                                      ensemble=mbd_mpc.plan_ensemble(self.args), ens_worst=a0.plan_worst)
         e.load_schedule(colds)   # sigma = 1.0 in every row (path_integral.py:140)
         return e
 

@@ -9,7 +9,9 @@ planner's recommended temperature for the env.  `zero` is the plant under zero a
 one line: the closed-loop mean reward over the seeds and the wall time of one warm control step of the whole batch.
 `--plant_friction` / `--plant_gear` run every algorithm and the zero-action baseline against a plant whose contact friction and
 actuator gear are scaled by those factors, while the planners keep the nominal model (DESIGN.md §5k).  `--plan_friction` /
-`--plan_gear` (K values each) let every algorithm plan against the ensemble of the K models (DESIGN.md §5l).
+`--plan_gear` (K values each) let every algorithm plan against the ensemble of the K models (DESIGN.md §5l).  `--plan_members K`
+with `--plan_friction_range lo hi` / `--plan_gear_range lo hi` draws the K members afresh at every control step instead, and
+`--plan_worst m` scores a sample by its m worst members rather than the mean of all K (DESIGN.md §5m).
 """
 from __future__ import annotations
 
@@ -38,6 +40,16 @@ class Args:
     plant_gear: float = 1.0  # the plant's actuator gear over the planners' model (xpbd envs)
     plan_friction: tuple[float, ...] = ()  # the planners' ensemble: member k's friction factor (xpbd envs; empty = nominal)
     plan_gear: tuple[float, ...] = ()  # member k's actuator-gear factor (as many as plan_friction)
+    plan_members: int = 0  # members drawn afresh at every control step (excludes plan_friction / plan_gear; 0 = none)
+    plan_friction_range: tuple[float, ...] = ()  # (lo, hi) of the drawn members' friction factors
+    plan_gear_range: tuple[float, ...] = ()  # (lo, hi) of the drawn members' actuator-gear factors
+    plan_worst: int = 0  # score a sample by the mean of its plan_worst worst member returns (0 = the mean of all)
+
+
+def plan_risk(args: Args) -> dict:
+    """the drawn-ensemble and risk-measure fields every algorithm's Args takes as they are"""
+    return dict(plan_members=args.plan_members, plan_friction_range=tuple(args.plan_friction_range),
+                plan_gear_range=tuple(args.plan_gear_range), plan_worst=args.plan_worst)
 
 
 def mbd_args(args: Args, seeds=SEEDS):
@@ -45,7 +57,7 @@ def mbd_args(args: Args, seeds=SEEDS):
     return [mbd_mpc.Args(seed=s, env_name=args.env_name, Nsample=args.Nsample, Hsample=args.Hsample, Ndiffuse=args.Nsolve,
                          Nwarm=args.Nwarm, Nstep=args.Nstep, temp_sample=temp, plant_friction=args.plant_friction,
                          plant_gear=args.plant_gear, plan_friction=tuple(args.plan_friction), plan_gear=tuple(args.plan_gear),
-                         not_render=True, disable_recommended_params=True)
+                         **plan_risk(args), not_render=True, disable_recommended_params=True)
             for s in seeds]
 
 
@@ -54,7 +66,8 @@ def pi_args(args: Args, method: str, seeds=SEEDS):
     return [pi_mpc.Args(seed=s, env_name=args.env_name, update_method=method, Nsample=args.Nsample, Hsample=args.Hsample,
                         Nrefine=args.Nsolve, Nwarm=args.Nwarm, Nstep=args.Nstep, sigma_warm=args.sigma_warm, temp_sample=temp,
                         plant_friction=args.plant_friction, plant_gear=args.plant_gear, plan_friction=tuple(args.plan_friction),
-                        plan_gear=tuple(args.plan_gear), not_render=True, disable_recommended_params=True) for s in seeds]
+                        plan_gear=tuple(args.plan_gear), **plan_risk(args), not_render=True, disable_recommended_params=True)
+            for s in seeds]
 
 
 def zero_action_rewards(env, states0: np.ndarray, Nstep: int, friction=1.0, gear=1.0) -> np.ndarray:
