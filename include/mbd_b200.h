@@ -6,6 +6,10 @@
  * device memory owned by the caller (torch tensors on the Python side); the stream is passed
  * explicitly; return 0 on success, a negative MBD_E* code otherwise (no exceptions cross the
  * ABI, nothing is allocated after *_create).  See INTEGRATION.md for the ctypes stub.
+ *
+ * The structs and constants Python uses from this header, mbd_model.h, mbd_kin64.h, mbd_sac.h and mbd_sac_learn.h are mirrored
+ * in mbd_b200/_lib.py and mbd_b200/model/blob.py; tests/test_abi.py compiles every mirror against these headers (offset, size
+ * and kind of every field, every constant), so a change here is made there too.
  */
 #ifndef MBD_B200_H_
 #define MBD_B200_H_
@@ -25,10 +29,6 @@ extern "C" {
 typedef struct mbd_model mbd_model;
 typedef void* mbd_stream; /* cudaStream_t */
 
-/* ABI/layout self-description (cross-checked against the Python packer in tests/test_abi.py) */
-int mbd_layout_info(int32_t* out, int n);
-/* sizeof / offsetof of the structs passed by pointer (mbd_step_params, mbd_step_ctl, mbd_step_plan), same cross-check */
-int mbd_abi_sizes(int32_t* out, int n);
 const char* mbd_last_error(void);
 int mbd_device_count(void);
 /* rollout kernel mapping: 0 = auto (by shard size), 1 = v1 (one link per lane), 2 / 3 = v2 (one link per warp, lane = sample)
@@ -210,11 +210,6 @@ typedef struct mbd_step_plan {
   int32_t ens_worst;                 /* 0 .. ens_k with a table (0 = the mean), 0 without */
 } mbd_step_plan;
 #define MBD_ENS_MAXK 16
-/* sizeof(mbd_step_plan), offsetof ens_factors_dev / ens_rews_dev / ens_k and MBD_ENS_MAXK (cross-checked against the ctypes mirror) */
-int mbd_ens_abi_sizes(int32_t* out, int n);
-/* sizeof(mbd_step_plan), offsetof ens_worst, sizeof(mbd_ens_draw_plan) and offsetof its keys_dev / ranges_dev / mpc_ctl_dev /
- * ens_factors_dev (cross-checked against the ctypes mirror) */
-int mbd_ens_risk_abi_sizes(int32_t* out, int n);
 /* Test entry point: the score launch of an ensemble step alone, on whatever the caller put into ens_rews_dev [count][K]:
  * rews_dev [count] <- the ordered mean (worst == 0) or the worst-m score (m = worst) of each row.  MBD_EINVAL before any CUDA call for a
  * NULL buffer, count < 1, K outside 1 .. MBD_ENS_MAXK or worst outside 0 .. K. */
@@ -273,8 +268,6 @@ typedef struct mbd_pi_bufs {        /* 24 bytes */
  * (xref), a missing buffer of the method, or a plan mbd_batch_step_launch would refuse. */
 int mbd_pi_batch_step_launch(const mbd_step_plan* plan, int B, int Nrefine, int method, const float* temps_dev,
                              const mbd_pi_bufs* bufs, int tail_only, mbd_stream s);
-/* sizeof / offsetof of mbd_pi_bufs (cross-checked against the ctypes mirror) */
-int mbd_pi_abi_sizes(int32_t* out, int n);
 /* ---- model-based diffusion as a black-box optimiser (upstream mbd/blackbox/mbd_opt.py:64-80) as the same three launches -------
  * B independent solves of one objective and shape in lockstep, laid out as mbd_batch_step_launch with H = 1 and nu = dim
  * (model, car_params, state_init and xref are not read and model / xref must be NULL).  Launch (1) (csrc/blackbox.cuh) draws
@@ -292,8 +285,6 @@ typedef struct mbd_bbo_bufs {        /* 24 bytes */
 } mbd_bbo_bufs;
 int mbd_bbo_batch_step_launch(const mbd_step_plan* plan, int B, int Ndiffuse, int fn, const float* temps_dev,
                               const mbd_bbo_bufs* bufs, mbd_stream s);
-/* sizeof / offsetof of mbd_bbo_bufs and the MBD_BBO_* values (cross-checked against the ctypes mirror) */
-int mbd_bbo_abi_sizes(int32_t* out, int n);
 
 /* ---- model-based diffusion over the weights of a 784-32-32-10 MLP (upstream mbd/blackbox/mbd_mnist.py) ---------------------
  * One solve (B = 1) laid out as mbd_batch_step_launch with H = 1 and nu = 26506 (the parameter row of csrc/mnist.cuh: W1
@@ -326,8 +317,6 @@ int mbd_mnist_forward(const float* Y0s_dev, int n_models, const mbd_mnist_bufs* 
  * scratch size needed to *scratch_bytes and returns.  Synchronous on the stream's work only (no host synchronisation). */
 int mbd_mnist_batch_indices(const uint32_t* sub_keys_host, int Ndiffuse, int n_data, int N, int32_t* idx_dev, void* scratch_dev,
                             size_t* scratch_bytes, mbd_stream s);
-/* sizeof / offsetof of mbd_mnist_bufs and MBD_MNIST_HNU (cross-checked against the ctypes mirror) */
-int mbd_mnist_abi_sizes(int32_t* out, int n);
 
 /* ---- a batch of environments stepped together on the device (vmap(env.reset) / vmap(env.step) with Brax's training wrappers) --
  * B environments of one kind, each with its own state, stepped by two launches: (1) the env's rollout kernel with H = 1 and a
@@ -387,8 +376,6 @@ int mbd_vec_step(const mbd_vec_plan* plan, mbd_stream s);
 int mbd_vec_set_state(const mbd_vec_plan* plan, mbd_stream s);
 /* xpbd envs: world link poses x.pos [B][L][3], x.rot [B][L][4] of the current states (PipelineEnv._make_pipeline_state) */
 int mbd_vec_world_poses(const mbd_vec_plan* plan, float* pos_dev, float* rot_dev, mbd_stream s);
-/* sizeof / offsetof of mbd_vec_plan and MBD_K64_WORDS (cross-checked against the ctypes mirror) */
-int mbd_vec_abi_sizes(int32_t* out, int n);
 
 /* ---- PPO on the vector env (Brax's ppo.train, v0.10.x line [brax-recalled]; mbd_b200/rl) ---------------------------------------
  * The acting step, the observation statistics and GAE on the device; the nets, the loss and Adam stay in torch.  A training step's
@@ -450,8 +437,6 @@ int mbd_ppo_obs_stats(const mbd_ppo_plan* plan, mbd_stream s);
 /* one launch per minibatch: compute_gae with the truncation mask on the trajectories traj_dev (rewards * reward_scaling), the
  * advantage normalisation (adv - mean) / (std + 1e-8) (population std) and the entropy noise */
 int mbd_ppo_gae(const mbd_ppo_plan* plan, mbd_stream s);
-/* sizeof / offsetof of mbd_ppo_plan and the MBD_PPO_* limits (cross-checked against the ctypes mirror) */
-int mbd_ppo_abi_sizes(int32_t* out, int n);
 
 /* ---- SAC on the vector env (Brax's sac.train, v0.10.x line [brax-recalled]; mbd_b200/rl/sac.py) ---------------------------------
  * The acting step, the replay ring and its uniform sampler on the device; the losses and the three Adam optimisers stay in torch.
@@ -500,8 +485,6 @@ int mbd_sac_record(const mbd_sac_plan* plan, mbd_stream s);
 /* one launch per training step: buffer key, sample key = split(buffer key); updates * batch randint indices in 0 .. size - 1 from
  * sample key, the gathered rows, and the three noise tensors of every update from noise_keys row s; s += 1 */
 int mbd_sac_sample(const mbd_sac_plan* plan, mbd_stream s);
-/* sizeof / offsetof of mbd_sac_plan and the MBD_SAC_* limits (cross-checked against the ctypes mirror) */
-int mbd_sac_abi_sizes(int32_t* out, int n);
 
 /* ---- the fused SAC gradient update (include/mbd_sac_learn.h, csrc/sac_learn.cuh) ---------------------------------------------
  * One Brax sgd_step on the batch and noise of update g = *upd_ctl_dev (the sampler's batch_dev / eps_dev of mbd_sac_plan): the three
@@ -537,8 +520,6 @@ typedef struct mbd_sac_learn_plan {
 int64_t mbd_sac_learn_scratch(int O, int nu, int batch);
 /* one sgd_step (two launches) */
 int mbd_sac_update(const mbd_sac_learn_plan* plan, mbd_stream s);
-/* sizeof / offsetof of mbd_sac_learn_plan and the limits (cross-checked against the ctypes mirror) */
-int mbd_sac_learn_abi_sizes(int32_t* out, int n);
 
 /* ---- model-based diffusion as a receding-horizon controller (mbd_b200/planners/mbd_mpc.py, DESIGN.md §5i) ----------------------
  * B closed loops of one env and shape, each planning with the buffers of mbd_batch_step_launch (params [B][Ndiffuse], ctl [B],
@@ -571,8 +552,6 @@ typedef struct mbd_mpc_plan {
   float* rew_hist_log_dev;         /* [B][Nstep]: rews.mean() of every control step's last diffusion step */
 } mbd_mpc_plan;
 int mbd_mpc_advance(const mbd_mpc_plan* plan, int mode, mbd_stream s);
-/* sizeof / offsetof of mbd_mpc_plan (cross-checked against the ctypes mirror) */
-int mbd_mpc_abi_sizes(int32_t* out, int n);
 
 /* ---- the path-integral baselines as receding-horizon controllers (mbd_b200/planners/pi_mpc.py, DESIGN.md §5j) -------------------
  * The same launch for B closed loops that plan with mbd_pi_batch_step_launch: base is the plan above with the baseline engine's
@@ -589,8 +568,6 @@ typedef struct mbd_mpc_pi_plan {
   float* sigma_log_dev;            /* [B][Nstep] */
 } mbd_mpc_pi_plan;
 int mbd_mpc_pi_advance(const mbd_mpc_pi_plan* plan, int mode, mbd_stream s);
-/* sizeof / offsetof of mbd_mpc_pi_plan (cross-checked against the ctypes mirror) */
-int mbd_mpc_pi_abi_sizes(int32_t* out, int n);
 
 /* Test / instrumentation entry point: launches (2) and (3) of mbd_step_launch only, on whatever the caller put into Y0s_dev,
  * rews_dev / logpd_dev (the symmetric-buffer slices when P > 1), Ybars_dev[i] and params_dev[i].  Same plan checks as

@@ -2,6 +2,9 @@
 
 The product path has NO CPU fallback: if the library is missing and cannot be built, or no
 CUDA device is present when a device entry point is called, this module raises.
+
+Each ctypes.Structure below mirrors the C struct named by its `_c_name_`, and the integer constants mirror the headers' MBD_*
+values; tests/test_abi.py compiles all of them against include/.
 """
 from __future__ import annotations
 
@@ -25,11 +28,13 @@ class MbdError(RuntimeError):
 
 class StepParams(ctypes.Structure):
     """mbd_step_params (include/mbd_b200.h): one row per diffusion step index, 32 bytes"""
+    _c_name_ = "mbd_step_params"
     _fields_ = [("key", ctypes.c_uint32 * 2), ("sigma", ctypes.c_float), ("coef", ctypes.c_float * 5)]
 
 
 class StepPlan(ctypes.Structure):
     """mbd_step_plan (include/mbd_b200.h), field for field"""
+    _c_name_ = "mbd_step_plan"
     _fields_ = [
         ("model", c_vp), ("car_params_dev", c_vp), ("state_init_dev", c_vp), ("params_dev", c_vp), ("ctl_dev", c_vp),
         ("Ybars_dev", c_vp), ("rew_hist_dev", c_vp),
@@ -48,16 +53,19 @@ class StepPlan(ctypes.Structure):
 
 class PiBufs(ctypes.Structure):
     """mbd_pi_bufs (include/mbd_b200.h): the buffers the path-integral update rules add to a step plan"""
+    _c_name_ = "mbd_pi_bufs"
     _fields_ = [("sigma_hist_dev", c_vp), ("cma_scratch_dev", c_vp), ("cem_idx_dev", c_vp)]
 
 
 class BboBufs(ctypes.Structure):
     """mbd_bbo_bufs (include/mbd_b200.h): what a black-box step adds to a step plan"""
+    _c_name_ = "mbd_bbo_bufs"
     _fields_ = [("init_keys_dev", c_vp), ("best_hist_dev", c_vp), ("x_min", ctypes.c_float), ("x_max", ctypes.c_float)]
 
 
 class MnistBufs(ctypes.Structure):
     """mbd_mnist_bufs (include/mbd_b200.h): what an MNIST step adds to a step plan"""
+    _c_name_ = "mbd_mnist_bufs"
     _fields_ = [("train_images_dev", c_vp), ("train_labels_dev", c_vp), ("test_images_dev", c_vp), ("test_labels_dev", c_vp),
                 ("keys_dev", c_vp), ("batch_idx_dev", c_vp), ("acc_hist_dev", c_vp), ("layers", ctypes.c_int32 * 4),
                 ("n_train", ctypes.c_int32), ("n_test", ctypes.c_int32), ("eval_every", ctypes.c_int32)]
@@ -65,6 +73,7 @@ class MnistBufs(ctypes.Structure):
 
 class VecPlan(ctypes.Structure):
     """mbd_vec_plan (include/mbd_b200.h): a batch of envs stepped together on the device"""
+    _c_name_ = "mbd_vec_plan"
     _fields_ = [("kind", ctypes.c_int32), ("B", ctypes.c_int32), ("model", c_vp), ("params_dev", c_vp), ("kin_dev", c_vp),
                 ("reset_dev", c_vp), ("obs_layout", ctypes.c_int32), ("done_rule", ctypes.c_int32), ("episode_length", ctypes.c_int32),
                 ("nq", ctypes.c_int32), ("nqd", ctypes.c_int32), ("nu", ctypes.c_int32),
@@ -75,6 +84,7 @@ class VecPlan(ctypes.Structure):
 
 class PpoPlan(ctypes.Structure):
     """mbd_ppo_plan (include/mbd_b200.h): the PPO acting step, observation statistics and GAE"""
+    _c_name_ = "mbd_ppo_plan"
     _fields_ = [("B", ctypes.c_int32), ("O", ctypes.c_int32), ("nu", ctypes.c_int32), ("slots", ctypes.c_int32),
                 ("unroll", ctypes.c_int32), ("mb", ctypes.c_int32), ("reward_scaling", ctypes.c_float), ("discount", ctypes.c_float),
                 ("gae_lambda", ctypes.c_float), ("act_key_rows", ctypes.c_int32), ("loss_key_rows", ctypes.c_int32),
@@ -88,6 +98,7 @@ class PpoPlan(ctypes.Structure):
 
 class SacPlan(ctypes.Structure):
     """mbd_sac_plan (include/mbd_b200.h): the SAC acting step, the replay record and the replay sampler"""
+    _c_name_ = "mbd_sac_plan"
     _fields_ = [("B", ctypes.c_int32), ("O", ctypes.c_int32), ("nu", ctypes.c_int32), ("capacity", ctypes.c_int32),
                 ("batch", ctypes.c_int32), ("updates", ctypes.c_int32), ("act_key_rows", ctypes.c_int32), ("noise_key_rows", ctypes.c_int32),
                 ("policy_dev", c_vp), ("mean_dev", c_vp), ("std_dev", c_vp), ("act_keys_dev", c_vp), ("act_ctl_dev", c_vp),
@@ -99,6 +110,7 @@ class SacPlan(ctypes.Structure):
 
 class SacLearnPlan(ctypes.Structure):
     """mbd_sac_learn_plan (include/mbd_b200.h): the fused SAC gradient update"""
+    _c_name_ = "mbd_sac_learn_plan"
     _fields_ = [("O", ctypes.c_int32), ("nu", ctypes.c_int32), ("batch", ctypes.c_int32), ("updates", ctypes.c_int32),
                 ("learning_rate", ctypes.c_float), ("reward_scaling", ctypes.c_float), ("discounting", ctypes.c_float),
                 ("tau", ctypes.c_float), ("policy_dev", c_vp), ("q_dev", c_vp), ("target_q_dev", c_vp), ("log_alpha_dev", c_vp),
@@ -109,6 +121,7 @@ class SacLearnPlan(ctypes.Structure):
 
 class MpcPlan(ctypes.Structure):
     """mbd_mpc_plan (include/mbd_b200.h): the step between two control steps of the receding-horizon controller"""
+    _c_name_ = "mbd_mpc_plan"
     _fields_ = [("B", ctypes.c_int32), ("H", ctypes.c_int32), ("nu", ctypes.c_int32), ("Ndiffuse", ctypes.c_int32),
                 ("Nwarm", ctypes.c_int32), ("Nstep", ctypes.c_int32), ("state_words", ctypes.c_int32), ("pad", ctypes.c_int32),
                 ("params_dev", c_vp), ("ctl_dev", c_vp), ("Ybars_dev", c_vp), ("rew_hist_dev", c_vp), ("keys_dev", c_vp),
@@ -118,11 +131,13 @@ class MpcPlan(ctypes.Structure):
 
 class MpcPiPlan(ctypes.Structure):
     """mbd_mpc_pi_plan (include/mbd_b200.h): mbd_mpc_plan for a path-integral baseline, plus the sigma reset and its log"""
+    _c_name_ = "mbd_mpc_pi_plan"
     _fields_ = [("base", MpcPlan), ("sigma_warm", ctypes.c_float), ("pad", ctypes.c_int32), ("sigma_log_dev", c_vp)]
 
 
 class EnsDrawPlan(ctypes.Structure):
     """mbd_ens_draw_plan (include/mbd_b200.h): the planner ensemble drawn afresh at every control step"""
+    _c_name_ = "mbd_ens_draw_plan"
     _fields_ = [("B", ctypes.c_int32), ("K", ctypes.c_int32), ("Nstep", ctypes.c_int32), ("pad", ctypes.c_int32),
                 ("keys_dev", c_vp), ("ranges_dev", c_vp), ("mpc_ctl_dev", c_vp), ("ens_factors_dev", c_vp)]
 
@@ -170,7 +185,6 @@ def lib():
     L = ctypes.CDLL(path)
     L.mbd_last_error.restype = ctypes.c_char_p
     L.mbd_device_count.restype = ctypes.c_int
-    L.mbd_layout_info.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_model_create.restype = c_vp
     L.mbd_model_create.argtypes = [c_u32p, ctypes.c_size_t]
     L.mbd_model_destroy.argtypes = [c_vp]
@@ -200,40 +214,29 @@ def lib():
     L.mbd_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, c_vp, c_vp]
     L.mbd_pi_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
                                            ctypes.POINTER(PiBufs), ctypes.c_int, c_vp]
-    L.mbd_pi_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
-    L.mbd_ens_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
-    L.mbd_ens_risk_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_ens_score.argtypes = [c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp]
     L.mbd_ens_draw.argtypes = [ctypes.POINTER(EnsDrawPlan), c_vp]
     L.mbd_bbo_batch_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp,
                                             ctypes.POINTER(BboBufs), c_vp]
-    L.mbd_bbo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_mnist_step_launch.argtypes = [ctypes.POINTER(StepPlan), ctypes.c_int, ctypes.POINTER(MnistBufs), c_vp]
     L.mbd_mnist_forward.argtypes = [c_vp, ctypes.c_int, ctypes.POINTER(MnistBufs), c_vp, ctypes.c_int, c_vp, c_vp, c_vp]
     L.mbd_mnist_batch_indices.argtypes = [c_u32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_vp, c_vp,
                                           ctypes.POINTER(ctypes.c_size_t), c_vp]
-    L.mbd_mnist_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_vec_reset.argtypes = [ctypes.POINTER(VecPlan), c_vp, c_vp]
     L.mbd_vec_step.argtypes = [ctypes.POINTER(VecPlan), c_vp]
     L.mbd_vec_set_state.argtypes = [ctypes.POINTER(VecPlan), c_vp]
     L.mbd_vec_world_poses.argtypes = [ctypes.POINTER(VecPlan), c_vp, c_vp, c_vp]
-    L.mbd_vec_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_ppo_act.argtypes = [ctypes.POINTER(PpoPlan), ctypes.c_int, c_vp]
     L.mbd_ppo_obs_stats.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
     L.mbd_ppo_gae.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
-    L.mbd_ppo_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_sac_act.argtypes = [ctypes.POINTER(SacPlan), ctypes.c_int, c_vp]
     L.mbd_sac_record.argtypes = [ctypes.POINTER(SacPlan), c_vp]
     L.mbd_sac_sample.argtypes = [ctypes.POINTER(SacPlan), c_vp]
-    L.mbd_sac_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_sac_learn_scratch.restype = ctypes.c_int64
     L.mbd_sac_learn_scratch.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int]
     L.mbd_sac_update.argtypes = [ctypes.POINTER(SacLearnPlan), c_vp]
-    L.mbd_sac_learn_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_mpc_advance.argtypes = [ctypes.POINTER(MpcPlan), ctypes.c_int, c_vp]
-    L.mbd_mpc_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_mpc_pi_advance.argtypes = [ctypes.POINTER(MpcPiPlan), ctypes.c_int, c_vp]
-    L.mbd_mpc_pi_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     L.mbd_step_launch_ev.argtypes =[ctypes.POINTER(StepPlan), c_vp, c_vp, c_vp, c_vp, c_vp]
     L.mbd_event_create.restype = c_vp
     L.mbd_event_destroy.argtypes = [c_vp]
@@ -242,14 +245,13 @@ def lib():
     L.mbd_event_elapsed_ms.restype = ctypes.c_float
     L.mbd_event_elapsed_ms.argtypes = [c_vp, c_vp]
     L.mbd_ffma_peak.argtypes = [c_vp, ctypes.c_int, c_f32p, c_vp]
-    L.mbd_abi_sizes.argtypes = [c_i32p, ctypes.c_int]
     _LIB = L
     return L
 
 
-EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_layout_info", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_pi_abi_sizes", "mbd_ens_abi_sizes", "mbd_ens_risk_abi_sizes", "mbd_ens_score", "mbd_ens_draw", "mbd_bbo_batch_step_launch", "mbd_bbo_abi_sizes", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_mnist_abi_sizes", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_abi_sizes", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_ppo_abi_sizes", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_abi_sizes", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_sac_learn_abi_sizes", "mbd_mpc_advance", "mbd_mpc_abi_sizes", "mbd_mpc_pi_advance", "mbd_mpc_pi_abi_sizes", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
-           "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak", "mbd_abi_sizes"]
+EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
+           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_ens_score", "mbd_ens_draw", "mbd_bbo_batch_step_launch", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_mpc_advance", "mbd_mpc_pi_advance", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak"]
 
 
 def check(rc: int, what: str):

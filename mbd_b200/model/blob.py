@@ -43,13 +43,6 @@ REWARD_HUMANOIDRUN, REWARD_HUMANOIDTRACK, REWARD_HOPPER, REWARD_HUMANOIDSTANDUP,
 _BIG = 3.0e38  # stands in for +-inf limits (keeps the arithmetic NaN-free)
 
 
-def layout_words():
-    """The numbers `mbd_layout_info` must return (ABI cross-check)."""
-    return [MAGIC, HDR_WORDS, NFIELDS, MAXL, MAXCHILD, MAXDOF, MAXCON, MAXTRACK, DOF_STRIDE, CON_STRIDE,
-            H_DT, H_RW0, F_MASS, F_COM, F_RC, F_JQ, F_RP, F_PQ, F_PARITY, F_SLIDE, F_DOF0, F_NCON, F_CON0,
-            BLOB_WORDS, STATE_STRIDE]
-
-
 def pack(sys: System, n_frames: int, reward: int, links=None, track_links=(), reward_params=(0, 0, 0, 0)) -> np.ndarray:
     """Returns the uint32 blob.  `links` optionally restricts the simulated links (humanoidtrack
     drops the 5 cosmetic, dynamically decoupled *_ref bodies, SURVEY App. B)."""

@@ -1,6 +1,5 @@
-"""Black-box solves without a device: mbd_bbo_batch_step_launch refuses bad arguments before any CUDA call (with a message), the
-mbd_bbo_bufs mirror matches the C struct, Args carries mbd_opt.py's constants, the key chain is mbd_opt.py's, and the saved
-curve has the reference's shape."""
+"""Black-box solves without a device: mbd_bbo_batch_step_launch refuses bad arguments before any CUDA call (with a message), Args
+carries mbd_opt.py's constants, the key chain is mbd_opt.py's, and the saved curve has the reference's shape."""
 import ctypes
 
 import numpy as np
@@ -69,15 +68,6 @@ def test_bbo_launch_null_plan_and_bufs_rejected():
     assert _reject(None)[0] == -1 and "plan is NULL" in _reject(None, bufs=_bufs())[1]
     rc, err = _reject(_plan(), bufs=None)
     assert rc == -1 and "bufs is NULL" in err, err
-
-
-def test_bbo_bufs_struct_matches_the_ctypes_mirror():
-    out = np.zeros(16, np.int32)
-    n = _lib.lib().mbd_bbo_abi_sizes(out.ctypes.data_as(_lib.c_i32p), 16)
-    B = _lib.BboBufs
-    assert n == 7
-    assert out[:4].tolist() == [ctypes.sizeof(B), B.best_hist_dev.offset, B.x_min.offset, B.x_max.offset]
-    assert out[4:7].tolist() == [_lib.BBO_FNS["Ackley"], _lib.BBO_FNS["Rastrigin"], _lib.BBO_FNS["Levy"]]
 
 
 def test_args_defaults_are_the_reference_constants():

@@ -1,5 +1,5 @@
-"""Worst-m scores and drawn members of the planner ensemble without a GPU (DESIGN.md §5m): the ctypes mirrors of ens_worst and of
-the draw plan, every C refusal (all before any CUDA call), the refusals of the engines and of the controllers' check_args, the member
+"""Worst-m scores and drawn members of the planner ensemble without a GPU (DESIGN.md §5m): ens_worst in the former pad word and the
+size of the draw plan, every C refusal (all before any CUDA call), the refusals of the engines and of the controllers' check_args, the member
 key chain, the numpy worst-m specification on constructed families, and the run_mpc driver."""
 import ctypes
 import itertools
@@ -17,14 +17,10 @@ FAKE = 0x1000   # never dereferenced: every case below fails validation, which r
 f32 = np.float32
 
 
-def test_abi_sizes_match_the_ctypes_mirrors():
-    out = (ctypes.c_int32 * 12)()
-    n = _lib.lib().mbd_ens_risk_abi_sizes(out, 12)
-    P, D = _lib.StepPlan, _lib.EnsDrawPlan
-    assert list(out[:n]) == [ctypes.sizeof(P), P.ens_worst.offset, ctypes.sizeof(D), D.keys_dev.offset, D.ranges_dev.offset,
-                             D.mpc_ctl_dev.offset, D.ens_factors_dev.offset]
+def test_ens_worst_takes_the_pad_word():
+    P = _lib.StepPlan
     assert P.ens_worst.offset == P.ens_k.offset + 4 and ctypes.sizeof(P) == P.ens_k.offset + 8   # the former pad word
-    assert ctypes.sizeof(D) == 48
+    assert ctypes.sizeof(_lib.EnsDrawPlan) == 48
 
 
 # ---- the C refusals -----------------------------------------------------------------------------------------------------------

@@ -177,14 +177,6 @@ def test_c_restatement_within_the_radius():
         assert abs(float(j) - r["J"]) <= r["rJ"]
 
 
-def test_abi_sizes():
-    out = (ctypes.c_int32 * 16)()
-    n = _lib.lib().mbd_mnist_abi_sizes(out, 16)
-    B = _lib.MnistBufs
-    assert list(out[:n]) == [ctypes.sizeof(B), B.keys_dev.offset, B.acc_hist_dev.offset, B.layers.offset, B.n_train.offset,
-                             B.eval_every.offset, _lib.MNIST_HNU]
-
-
 def test_argument_rejection():
     L = _lib.lib()
     plan = _lib.StepPlan()

@@ -1,4 +1,4 @@
-"""The receding-horizon controller without a GPU: its key table, the shift, the argument checks, the ABI of mbd_mpc_advance and the
+"""The receding-horizon controller without a GPU: its key table, the shift, the argument checks, the refusals of mbd_mpc_advance and the
 CPU restatement of the controller on the oracle (tests/mpc_ref.py)."""
 import ctypes
 
@@ -111,15 +111,6 @@ def test_recommended_params_are_applied_first(monkeypatch):
 
 
 # ---- the C ABI --------------------------------------------------------------------------------------------------------------
-def test_mpc_plan_matches_the_ctypes_mirror():
-    out = np.zeros(16, np.int32)
-    n = _lib.lib().mbd_mpc_abi_sizes(out.ctypes.data_as(_lib.c_i32p), 16)
-    P = _lib.MpcPlan
-    exp = [ctypes.sizeof(P), P.state_words.offset, P.params_dev.offset, P.keys_dev.offset, P.env_actions_dev.offset,
-           P.rew_hist_log_dev.offset, _lib.MPC_ACT, _lib.MPC_RECORD]
-    assert n == len(exp) and out[:n].tolist() == exp
-
-
 BUFS = ("params_dev", "ctl_dev", "Ybars_dev", "rew_hist_dev", "keys_dev", "mpc_ctl_dev", "env_actions_dev", "env_state_dev",
         "env_reward_dev", "actions_dev", "rewards_dev", "states_dev", "rew_hist_log_dev")
 ACT_BUFS = set(BUFS) - {"env_reward_dev", "rewards_dev"}

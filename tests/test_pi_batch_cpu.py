@@ -1,6 +1,6 @@
 """Batched path-integral solves without a device: mbd_pi_batch_step_launch refuses bad arguments before any CUDA call (with a
-message), run_path_integral_batch checks its Args before touching the device, the mbd_pi_bufs mirror matches the C struct, and
-run_mbd's --pi_batch builds the same sweeps as the sequential path."""
+message), run_path_integral_batch checks its Args before touching the device, mbd_pi_bufs is 24 bytes, a CEM index row holds the
+picks and their count, and run_mbd's --pi_batch builds the same sweeps as the sequential path."""
 import ctypes
 
 import numpy as np
@@ -75,14 +75,8 @@ def test_pi_tail_only_skips_the_env_checks_only():
     assert rc == -1 and "a work buffer is NULL" in err, err
 
 
-def test_pi_bufs_struct_matches_the_ctypes_mirror():
-    out = np.zeros(16, np.int32)
-    n = _lib.lib().mbd_pi_abi_sizes(out.ctypes.data_as(_lib.c_i32p), 16)
-    B = _lib.PiBufs
-    exp = [ctypes.sizeof(B), B.cma_scratch_dev.offset, B.cem_idx_dev.offset, _lib.PI_IDX_STRIDE, _lib.PI_METHODS["mppi"],
-           _lib.PI_METHODS["cma-es"], _lib.PI_METHODS["cem"]]
-    assert n == len(exp) and out[:n].tolist() == exp
-    assert ctypes.sizeof(B) == 24 and _lib.PI_IDX_STRIDE > _lib.PI_TOPK
+def test_pi_bufs_size_and_cem_slots():
+    assert ctypes.sizeof(_lib.PiBufs) == 24 and _lib.PI_IDX_STRIDE > _lib.PI_TOPK
 
 
 def _args(**kw):

@@ -1,5 +1,5 @@
-"""The receding-horizon controller of the path-integral baselines without a GPU: its key table, the argument checks, the ABI of
-mbd_mpc_pi_advance and the CPU restatement of the controller on the oracle (tests/pi_mpc_ref.py)."""
+"""The receding-horizon controller of the path-integral baselines without a GPU: its key table, the argument checks, the refusals
+of mbd_mpc_pi_advance and the CPU restatement of the controller on the oracle (tests/pi_mpc_ref.py)."""
 import ctypes
 
 import numpy as np
@@ -129,12 +129,8 @@ def test_comparison_driver_gives_every_algorithm_the_same_problem():
 
 
 # ---- the C ABI --------------------------------------------------------------------------------------------------------------
-def test_mpc_pi_plan_matches_the_ctypes_mirror():
-    out = np.zeros(16, np.int32)
-    n = _lib.lib().mbd_mpc_pi_abi_sizes(out.ctypes.data_as(_lib.c_i32p), 16)
+def test_mpc_pi_plan_extends_mpc_plan():
     P = _lib.MpcPiPlan
-    exp = [ctypes.sizeof(P), P.base.offset, P.sigma_warm.offset, P.sigma_log_dev.offset]
-    assert n == len(exp) and out[:n].tolist() == exp
     assert P.base.offset == 0 and P.sigma_warm.offset == ctypes.sizeof(_lib.MpcPlan)
 
 

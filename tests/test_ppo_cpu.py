@@ -295,14 +295,6 @@ def test_act_unknown_mode():
     assert "unknown mode" in L.mbd_last_error().decode()
 
 
-def test_abi_sizes_match_ctypes():
-    out = (ctypes.c_int32 * 16)()
-    n = _lib.lib().mbd_ppo_abi_sizes(out, 16)
-    P = _lib.PpoPlan
-    assert list(out[:n]) == [ctypes.sizeof(P), P.reward_scaling.offset, P.policy_dev.offset, P.env_obs_dev.offset, P.stat_dev.offset,
-                             P.ent_eps_dev.offset, _lib.PPO_MAX_OBS, _lib.PPO_MAX_NU, _lib.PPO_MAX_MB, _lib.PPO_STAT_ROWS]
-
-
 # ---- CLI ---------------------------------------------------------------------------------------------------------------------------
 def test_cli_hopper_says_sac_is_not_built():
     with pytest.raises(SystemExit, match="SAC"):

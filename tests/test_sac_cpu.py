@@ -355,14 +355,6 @@ def test_sample_rejected_before_cuda(fields, msg):
     assert msg in L.mbd_last_error().decode()
 
 
-def test_abi_sizes_match_ctypes():
-    out = (ctypes.c_int32 * 16)()
-    n = _lib.lib().mbd_sac_abi_sizes(out, 16)
-    P = _lib.SacPlan
-    assert list(out[:n]) == [ctypes.sizeof(P), P.noise_key_rows.offset, P.policy_dev.offset, P.env_obs_dev.offset, P.ring_dev.offset,
-                             P.eps_dev.offset, _lib.SAC_MAX_CAPACITY, _lib.SAC_HIDDEN]
-
-
 # ---- CLI ---------------------------------------------------------------------------------------------------------------------------
 def test_cli_ppo_env_points_to_train_brax():
     with pytest.raises(SystemExit, match="train_brax"):

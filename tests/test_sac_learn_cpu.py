@@ -1,6 +1,6 @@
 """The fused SAC update without a GPU: include/mbd_sac_learn.h's host harness (g++ -ffp-contract=off, the kernel's association
 orders) against the float64 contract of tests/sac_learn_ref.py on the families of tests/sac_learn_families.py, Adam and Polyak
-against float64, the deliberate mistakes of an fp32 mirror, the ABI's sizes and refusals, and the learner options."""
+against float64, the deliberate mistakes of an fp32 mirror, the ABI's refusals, and the learner options."""
 import ctypes
 import os
 import subprocess
@@ -229,16 +229,6 @@ def test_mistakes_leave_the_bound(mistake):
 
 
 # ---- ABI, refusals, options -----------------------------------------------------------------------------------------------------------
-def test_abi_sizes():
-    from mbd_b200 import _lib
-    L = _lib.lib()
-    out = (ctypes.c_int32 * 16)()
-    n = L.mbd_sac_learn_abi_sizes(out, 16)
-    P = _lib.SacLearnPlan
-    assert list(out[:n]) == [ctypes.sizeof(P), P.learning_rate.offset, P.policy_dev.offset, P.ctl_dev.offset, P.upd_ctl_dev.offset,
-                             P.scratch_floats.offset, P.losses_dev.offset, _lib.SAC_LEARN_MAX_BATCH, _lib.SAC_HIDDEN]
-
-
 def test_scratch_size_matches_harness(harness):
     from mbd_b200 import ops
     out = ctypes.c_longlong()
