@@ -27,14 +27,13 @@ import math
 import os
 import struct
 from dataclasses import dataclass
-from types import SimpleNamespace
 from typing import Optional
 
 import numpy as np
 import torch
 
 from mbd_b200 import _lib, ops, prng
-from mbd_b200.planners.engine import BatchedDiffusionEngine, make_schedule, pack_step_params
+from mbd_b200.planners.engine import LaunchInputs, StepEngine, make_schedule, pack_step_params
 
 LAYERS = (784, 32, 32, 10)
 HNU = 26506
@@ -226,26 +225,18 @@ def step_keys(seed: int, Ndiffuse: int):
 
 
 # ---- device engine -----------------------------------------------------------------------------------------------------------
-class MnistEngine(BatchedDiffusionEngine):
+class MnistEngine(StepEngine):
     """One MNIST solve (B = 1, H = 1, HNu = 26506) stepped by `mbd_mnist_step_launch`; the solve-level surface of
-    BatchedDiffusionEngine (set_step, step, capture, check_exchange).  Ybars[0][t] = the mean before step t (row Ndiffuse - 1 =
+    StepEngine (set_step, step, capture, check_exchange, solve).  Ybars[0][t] = the mean before step t (row Ndiffuse - 1 =
     the init), rew_hist[0][t] = Js.mean() of step t, acc_hist[t] = train / test correct-counts of the mean after step t (-1
     where not evaluated)."""
 
     def __init__(self, data, Nsample: int, temp: float, Ndiffuse: int, eval_every: int = 1, device: Optional[torch.device] = None):
-        self.B, self.N, self.H, self.Nu, self.HNu, self.Nd = 1, int(Nsample), 1, HNU, HNU, int(Ndiffuse)
         train_x, train_y, test_x, test_y = data
-        if self.Nd < 2:
-            raise ValueError("Ndiffuse must be at least 2")
-        if not 1 <= self.N <= len(train_x):
+        if not 1 <= int(Nsample) <= len(train_x):
             raise ValueError(f"Nsample must lie in 1 .. {len(train_x)} (the minibatch has Nsample images)")
-        self.env = SimpleNamespace(kind="mnist")
-        self.enable_demo = False
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.model = self.params_car = self.state_init = self.xref = None
-        self.rew_xref = 0.0
-        self._alloc([temp])
-        self._plan_c.temp = float(temp)   # launch (3) reads the plan's temperature (the batched plan leaves it 0)
+        # launch (3) reads the plan's temperature
+        super().__init__(LaunchInputs.none(), Nsample, 1, HNU, Ndiffuse, False, B=1, temp=temp, device=device)
         d = self.device
         u8 = lambda a: torch.from_numpy(np.array(a, np.uint8, copy=True)).to(d)   # noqa: E731
         self.train_x, self.train_y, self.test_x, self.test_y = u8(train_x), u8(train_y), u8(test_x), u8(test_y)
@@ -292,16 +283,13 @@ def run_mnist(args: Args, data=None, progress: bool = False):
     eng = MnistEngine(data, args.Nsample, args.temp_sample, args.Ndiffuse, args.eval_every)
     sigmas = make_schedule(args.beta0, args.betaT, args.Ndiffuse)[3]
     eng.load_schedule(args.seed, sigmas, params_to_row(init_params(args.seed)))
-    eng.set_step(args.Ndiffuse - 1)
-    if os.environ.get("MBD_GRAPH", "1") != "0":
-        eng.capture()   # the warm-up step is re-run from the same state; launch (1) re-zeroes the counts it adds to
-    for t in range(args.Ndiffuse - 1, 0, -1):
-        eng.step()
-        if progress and ((args.Ndiffuse - 1 - t) % args.log_every == args.log_every - 1 or t == 1):
-            acc = eng.acc_hist[t].cpu().numpy()
-            print(f"step {t}: J={eng.rew_hist[0, t].item():.2f}, train_acc={acc[0] / eng.n_train:.3f}, "
-                  f"test_acc={acc[1] / eng.n_test:.3f}", flush=True)
-    eng.check_exchange()
+
+    def log(t):
+        acc = eng.acc_hist[t].cpu().numpy()
+        print(f"step {t}: J={eng.rew_hist[0, t].item():.2f}, train_acc={acc[0] / eng.n_train:.3f}, "
+              f"test_acc={acc[1] / eng.n_test:.3f}", flush=True)
+    # the warm-up step of the capture is re-run from the same state; launch (1) re-zeroes the counts it adds to
+    eng.solve(log if progress else None, args.log_every)
     acc = eng.acc_hist[1:].flip(0).cpu().numpy().astype(np.float64)
     acc[acc < 0] = np.nan
     return dict(J=eng.rew_hist[0, 1:].flip(0).cpu().numpy(), train_acc=acc[:, 0] / eng.n_train, test_acc=acc[:, 1] / eng.n_test,

@@ -25,7 +25,6 @@ from __future__ import annotations
 
 import os
 from dataclasses import dataclass
-from types import SimpleNamespace
 from typing import Optional, Sequence
 
 import numpy as np
@@ -33,12 +32,7 @@ import torch
 
 import mbd_b200
 from mbd_b200 import _lib, ops, prng
-from mbd_b200.planners.engine import BatchedDiffusionEngine, key_chain, make_schedule, pack_step_params
-
-try:
-    from tqdm import tqdm
-except Exception:  # noqa: BLE001
-    tqdm = None
+from mbd_b200.planners.engine import LaunchInputs, StepEngine, key_chain, make_schedule, pack_step_params
 
 
 @dataclass
@@ -69,29 +63,21 @@ def sample_counts(args: Args) -> np.ndarray:
     return np.arange(1, args.Ndiffuse, dtype=np.int64) * args.Nsample
 
 
-class BboEngine(BatchedDiffusionEngine):
+class BboEngine(StepEngine):
     """B independent black-box solves of one objective and shape (Nsample, dim, Ndiffuse) stepped in lockstep by ONE
-    three-launch step (`mbd_bbo_batch_step_launch`); the solve-level surface of BatchedDiffusionEngine (set_step, step, capture,
-    check_exchange).  Ybars[b] holds problem b's means (row t = mu_0t of step t, row t - 1 its result; row Ndiffuse - 1 is not
+    three-launch step (`mbd_bbo_batch_step_launch`); the solve-level surface of StepEngine (set_step, step, capture,
+    check_exchange, solve).  Ybars[b] holds problem b's means (row t = mu_0t of step t, row t - 1 its result; row Ndiffuse - 1 is not
     read: the first step draws its mean per sample from init_keys[b]); rews[b] = J of the last step; best_hist[b][t] = Js.max()
     of step t (-inf before it runs)."""
 
     def __init__(self, fn_name: str, dim: int, Nsample: int, temps, Ndiffuse: int, device: Optional[torch.device] = None):
         if fn_name not in _lib.BBO_FNS:
             raise KeyError(fn_name)
-        self.B = len(temps)
-        if self.B < 1:
+        if len(temps) < 1:
             raise ValueError("a black-box batch needs at least one problem")
         self.fn_name, self.fn = fn_name, _lib.BBO_FNS[fn_name]
-        self.env = SimpleNamespace(kind="bbo")      # no env: launch (1) is the objective, the plan carries no model or table
-        self.N, self.H, self.Nu, self.HNu, self.Nd = int(Nsample), 1, int(dim), int(dim), int(Ndiffuse)
-        if self.Nd < 2:
-            raise ValueError("Ndiffuse must be at least 2")
-        self.enable_demo = False
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.model = self.params_car = self.state_init = self.xref = None
-        self.rew_xref = 0.0
-        self._alloc(temps)
+        # no env: launch (1) is the objective, the plan carries no model or table
+        super().__init__(LaunchInputs.none(), Nsample, 1, dim, Ndiffuse, False, B=len(temps), temps=temps, device=device)
         self.init_keys = torch.zeros((self.B, 2), device=self.device, dtype=torch.int32)
         self.best_hist = torch.full((self.B, self.Nd), float("-inf"), device=self.device)
         self.x_min, self.x_max = DOMAINS[fn_name]
@@ -134,16 +120,11 @@ def run_exp_batch(args: Args, seeds: Sequence[int], log_every: int = 10, progres
     sigmas = make_schedule(args.beta0, args.betaT, args.Ndiffuse)[3]
     pk = [problem_keys(s, args.Ndiffuse) for s in seeds]
     eng.load_schedule([k for k, _ in pk], sigmas, [k0 for _, k0 in pk])
-    eng.set_step(args.Ndiffuse - 1)
-    if os.environ.get("MBD_GRAPH", "1") != "0":
-        eng.capture()   # its warm-up step is re-run from the same state: every output is rewritten, best_hist is a max
-    steps = range(args.Ndiffuse - 1, 0, -1)
-    pbar = tqdm(steps, desc=f"Diffusing x{eng.B}") if (progress and tqdm is not None) else None
-    for n_done, t in enumerate(pbar if pbar is not None else steps):
-        eng.step()
-        if pbar is not None and (n_done % log_every == log_every - 1 or t == 1):
-            pbar.set_postfix({"rew": f"{eng.best_hist[:, t].mean().item():.2e}"})   # Js.max(), mean over the seeds
-    eng.check_exchange()
+
+    def log(t):
+        return {"rew": f"{eng.best_hist[:, t].mean().item():.2e}"}   # Js.max(), mean over the seeds
+    # the warm-up step of the capture is re-run from the same state: every output is rewritten, best_hist is a max
+    eng.solve(log if progress else None, log_every, f"Diffusing x{eng.B}" if progress else None)
     ys = eng.best_hist[:, 1:].flip(1).cpu().numpy()
     mus = eng.Ybars[:, 0].cpu().numpy()
     return sample_counts(args), ys, mus

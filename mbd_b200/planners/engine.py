@@ -17,6 +17,7 @@ on the path (NCCL only bootstraps the rendezvous of the symmetric buffer).
 from __future__ import annotations
 
 import ctypes
+import dataclasses
 import os
 from typing import Optional
 
@@ -25,6 +26,11 @@ import torch
 
 from .. import _lib, ops, prng
 from .sharding import ShardPlan
+
+try:  # tqdm is cosmetic
+    from tqdm import tqdm
+except Exception:  # noqa: BLE001
+    tqdm = None
 
 
 def linspace_f32(start: float, stop: float, num: int) -> np.ndarray:
@@ -84,24 +90,48 @@ def pack_step_params(keys: np.ndarray, sigmas: np.ndarray, alphas: Optional[np.n
     return tab.view(np.int32)
 
 
-def env_tensors(env, state_init, enable_demo: bool, d: torch.device):
-    """(model, params_car, state_init, xref) of one env on device d: what launch (1) of a step reads.  model is the
-    device-resident blob of a Brax-positional env (None for car2d / pushT, whose table is params_car); xref is the
-    demonstration when enable_demo is set."""
-    if env.kind == "xpbd":
-        raw = state_init.pipeline_state.raw if hasattr(state_init, "pipeline_state") else state_init
-        xref = torch.as_tensor(env.xref, device=d).contiguous() if enable_demo else None
-        return env.device_model(d), None, torch.as_tensor(np.ascontiguousarray(raw, dtype=np.float32), device=d), xref
-    if env.kind == "car2d":
-        params_car, xref = env.device_params()
-        x0 = state_init.pipeline_state if hasattr(state_init, "pipeline_state") else state_init
-        return None, params_car, torch.as_tensor(np.ascontiguousarray(x0, dtype=np.float32), device=d), (xref if enable_demo else None)
-    if env.kind == "pusht":
-        if enable_demo:
+@dataclasses.dataclass(frozen=True)
+class LaunchInputs:
+    """What launch (1) of a step reads besides the step buffers, on the device: the model blob of a Brax-positional env (None
+    for car2d / pushT, whose table is params_car), the initial state (one per problem of a batch), the demonstration (None
+    without a demo) and its reward offset, and env_kind, which picks the flat-state env when there is no model.
+
+    `none()` is the form of an engine whose launch (1) reads no env: the black-box objective, MNIST, and engines that drive
+    launches 2 and 3 on constructed inputs.  Launch (2) blends the demo in whenever xref is set and reads nothing else of it,
+    so such an engine runs a demo tail with any placeholder xref."""
+    model: Optional[object] = None
+    params_car: Optional[torch.Tensor] = None
+    state_init: Optional[torch.Tensor] = None
+    xref: Optional[torch.Tensor] = None
+    rew_xref: float = 0.0
+    env_kind: int = _lib.ENV_CAR2D
+
+    @classmethod
+    def none(cls) -> "LaunchInputs":
+        return cls()
+
+    @classmethod
+    def of_env(cls, env, state_init, enable_demo: bool, d: torch.device, batch: bool = False) -> "LaunchInputs":
+        """the inputs of env on device d from one initial state, or with batch from a list of them (state_init [B, state]; the
+        problems share the tables and the demonstration).  xref is the demonstration when enable_demo is set."""
+        if batch:
+            per = [cls.of_env(env, s, enable_demo, d) for s in state_init]
+            return dataclasses.replace(per[0], state_init=torch.stack([p.state_init for p in per]).contiguous())
+        if env.kind == "pusht" and enable_demo:
             raise ValueError("pushT has no demonstration (mbd_planner.py:118 applies to humanoidtrack / car2d)")
-        raw = state_init.pipeline_state.raw if hasattr(state_init, "pipeline_state") else state_init
-        return None, env.device_params(), torch.as_tensor(np.ascontiguousarray(raw, dtype=np.float32), device=d), None
-    raise ValueError(env.kind)
+        if env.kind not in ("xpbd", "car2d", "pusht"):
+            raise ValueError(env.kind)
+        if hasattr(state_init, "pipeline_state"):
+            state_init = state_init.pipeline_state if env.kind == "car2d" else state_init.pipeline_state.raw
+        x0 = torch.as_tensor(np.ascontiguousarray(state_init, dtype=np.float32), device=d)
+        rew_xref = float(getattr(env, "rew_xref", 0.0))
+        if env.kind == "xpbd":
+            xref = torch.as_tensor(env.xref, device=d).contiguous() if enable_demo else None
+            return cls(env.device_model(d), None, x0, xref, rew_xref)
+        if env.kind == "car2d":
+            params_car, xref = env.device_params()
+            return cls(None, params_car, x0, xref if enable_demo else None, rew_xref)
+        return cls(None, env.device_params(), x0, None, rew_xref, _lib.ENV_PUSHT)
 
 
 def ensemble_table(table, B: int, env, enable_demo: bool) -> np.ndarray:
@@ -136,76 +166,59 @@ def check_ens_worst(worst, K: Optional[int]) -> int:
     return int(worst)
 
 
-def xref_len(env, xref) -> int:
-    """href of the step plan: the demonstration's length in steps (0 without one)"""
-    return 0 if xref is None else int(xref.shape[1] if env.kind == "xpbd" else xref.shape[0])
 
 
-class DiffusionEngine:
-    def __init__(self, env, Nsample: int, Hsample: int, temp_sample: float, enable_demo: bool, state_init,
-                 device: Optional[torch.device] = None, group=None, Ndiffuse: int = 2, emulate=None):
-        """emulate = (P, rank, bufs): rank `rank` of P ranks that all live on THIS device and exchange through the plain
-        device buffers `bufs` (one per rank) — the same kernels, flags and peer loads as a real sharded run, used by the
-        single-GPU tests (`make_emulated_ranks`)."""
-        self.env = env
-        self.N, self.H, self.temp = int(Nsample), int(Hsample), float(temp_sample)
-        self.enable_demo = bool(enable_demo)
-        self.plan = ShardPlan.from_env(self.N, group) if emulate is None else ShardPlan(self.N, emulate[0], emulate[1], None)
-        self.group, self.P, self.rank = group, self.plan.P, self.plan.rank
-        self.n_local, self.n_begin = self.plan.n_local, self.plan.n_begin
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.Nu = env.action_size
+def _device(device) -> torch.device:
+    return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+
+
+class StepEngine:
+    """The device buffers and the C plan of a three-launch step, and the solve-level API on them.  One solve (B None) or B
+    independent solves stepped in lockstep (B >= 1), whose every per-problem buffer is [B, ...] with problem b's single-solve
+    block at index b.  A subclass says how a step is launched (`_launch`) and adds the fields of its own to the plan.  P and rank
+    are those of a sharded DiffusionEngine rank.
+
+    temp: the plan's temperature; temps: a batch's per-problem temperatures (a [B] device tensor the batched launches read in
+    its place).  n_begin / n_local: the samples of this rank (all N by default).  exchange: (rews, logpd, partial) of a sharded
+    rank, slices of the buffer its peers read; rews_all / logpd_all then gather every rank's samples."""
+
+    P, rank, group = 1, 0, None
+
+    def __init__(self, inputs: LaunchInputs, N: int, H: int, Nu: int, Ndiffuse: int, enable_demo: bool, B: Optional[int] = None,
+                 temp: float = 0.0, temps=None, device: Optional[torch.device] = None, n_begin: int = 0,
+                 n_local: Optional[int] = None, exchange=None):
+        self.N, self.H, self.Nu, self.Nd, self.B = int(N), int(H), int(Nu), int(Ndiffuse), B
+        if self.Nd < 2:
+            raise ValueError("Ndiffuse must be at least 2")
         self.HNu = self.H * self.Nu
-        self.Nd = max(int(Ndiffuse), 2)
-        d = self.device
+        self.enable_demo, self.temp = bool(enable_demo), float(temp)
+        self.n_begin, self.n_local = int(n_begin), self.N if n_local is None else int(n_local)
+        self.device = d = _device(device)
+        self.model, self.params_car, self.state_init, self.xref = inputs.model, inputs.params_car, inputs.state_init, inputs.xref
+        self.rew_xref, self.env_kind = inputs.rew_xref, inputs.env_kind
         f = dict(device=d, dtype=torch.float32)
-        self.Y0s = torch.empty((self.n_local, self.HNu), **f)
-        # ---- exchange: P > 1 needs ONE peer-mapped symmetric buffer per rank, [rews n_local | logpd n_local | partial HNu |
-        #      2 flag rows of 8 words]; the tail kernels read the peers' slices over NVLink themselves.
-        self.sym, self.peer_ptrs = None, None
-        self.exchange = "none" if self.P == 1 else "p2p"
-        self.off_rews, self.off_logpd, self.off_partial = 0, self.n_local, 2 * self.n_local
-        self.off_flags = 2 * self.n_local + self.HNu
-        if self.P > 1 and emulate is not None:
-            self.exchange = "p2p-emulated"
-            self.sym = emulate[2][self.rank]
-            assert self.sym.numel() == 2 * self.n_local + self.HNu + 16 and self.sym.device == d
-            self.peer_ptrs = (ctypes.c_uint64 * self.P)(*[int(b.data_ptr()) for b in emulate[2]])
-        elif self.P > 1:
-            import torch.distributed as dist
-            import torch.distributed._symmetric_memory as symm_mem
-            words = 2 * self.n_local + self.HNu + 16
-            self.sym = symm_mem.empty(words, dtype=torch.float32, device=d)
-            self.sym.zero_()
-            self.sym_hdl = symm_mem.rendezvous(self.sym, dist.group.WORLD if group is None else group)
-            self.peer_ptrs = (ctypes.c_uint64 * self.P)(*[int(p) for p in self.sym_hdl.buffer_ptrs])
-            torch.cuda.synchronize()
-            dist.barrier(group=group)
-        if self.P > 1:
-            self.rews_local = self.sym[self.off_rews:self.off_rews + self.n_local]
-            self.logpd_local = self.sym[self.off_logpd:self.off_logpd + self.n_local] if self.enable_demo else None
-            self.partial = self.sym[self.off_partial:self.off_partial + self.HNu]
+        lead, nl, HNu = (() if B is None else (B,)), self.n_local, self.HNu
+        self.temps = None if temps is None else torch.tensor(np.asarray(temps, np.float32), device=d)
+        self.Y0s = torch.empty(lead + (nl, HNu), **f)
+        if exchange is None:
+            self.rews = torch.empty(lead + (nl,), **f)
+            self.logpd = torch.empty(lead + (nl,), **f) if self.enable_demo else None
+            self.partial = torch.empty(HNu, **f)                 # read by sharded steps only; the plan requires it
+            self.rews_all, self.logpd_all = self.rews, self.logpd
+        else:
+            self.rews, self.logpd, self.partial = exchange
             self.rews_all = torch.empty(self.N, **f)
             self.logpd_all = torch.empty(self.N, **f) if self.enable_demo else None
-        else:
-            self.rews_local = torch.empty(self.n_local, **f)
-            self.logpd_local = torch.empty(self.n_local, **f) if self.enable_demo else None
-            self.partial = torch.empty(self.HNu, **f)
-            self.rews_all, self.logpd_all = self.rews_local, self.logpd_local
-        self.weights = torch.empty(self.n_local, **f)
-        self.scalars = torch.zeros(4, **f)
-        self.logp_scratch = torch.empty(self.N, **f)
-        self.run_scratch = torch.empty(((self.n_local + ops.RUN - 1) // ops.RUN) * self.HNu, **f)
+        self.logp_scratch = torch.empty(lead + (self.N,), **f)
+        self.weights = torch.empty(lead + (nl,), **f)
+        self.scalars = torch.zeros(lead + (4,), **f)
+        self.run_scratch = torch.empty(lead + ((nl + ops.RUN - 1) // ops.RUN, HNu), **f)
         # ---- device-resident solve state
-        self.Ybars = torch.zeros((self.Nd, self.HNu), **f)        # row i = input of step i, row i-1 = its output (row Nd-1 = YN = 0)
-        self.rew_hist = torch.zeros(self.Nd, **f)                 # rews.mean() of step i
-        self.params = torch.zeros((self.Nd, _lib.STEP_PARAMS_WORDS), device=d, dtype=torch.int32)
-        self.ctl = torch.zeros(_lib.STEP_CTL_WORDS, device=d, dtype=torch.int32)
-        self.launches_per_step = 3
-        self.launches_last_step = 3
+        self.Ybars = torch.zeros(lead + (self.Nd, HNu), **f)     # row i = input of step i, row i-1 = its output (row Nd-1 = YN = 0)
+        self.rew_hist = torch.zeros(lead + (self.Nd,), **f)      # rews.mean() of step i
+        self.params = torch.zeros(lead + (self.Nd, _lib.STEP_PARAMS_WORDS), device=d, dtype=torch.int32)
+        self.ctl = torch.zeros(lead + (_lib.STEP_CTL_WORDS,), device=d, dtype=torch.int32)
         self.graph = None
-        self.model, self.params_car, self.state_init, self.xref = env_tensors(env, state_init, self.enable_demo, d)
-        self.rew_xref = float(getattr(env, "rew_xref", 0.0))
         self._plan_c = self._make_plan()
 
     # ---- C-ABI plan ----------------------------------------------------------------------------------------------
@@ -213,25 +226,144 @@ class DiffusionEngine:
         p = _lib.StepPlan()
         vp = lambda t: None if t is None else t.data_ptr()   # noqa: E731
         p.model = self.model._h if self.model is not None else None
-        p.car_params_dev = vp(self.params_car)
-        p.state_init_dev = vp(self.state_init)
+        p.car_params_dev, p.state_init_dev, p.env_kind = vp(self.params_car), vp(self.state_init), self.env_kind
+        p.xref_dev, p.rew_xref = vp(self.xref), self.rew_xref
+        p.href = 0 if self.xref is None else int(self.xref.shape[-2])   # xref [href, 2] (car2d) or [ntrack, href, 3] (xpbd)
         p.params_dev, p.ctl_dev, p.Ybars_dev, p.rew_hist_dev = vp(self.params), vp(self.ctl), vp(self.Ybars), vp(self.rew_hist)
         p.n_total, p.n_begin, p.n_local, p.H, p.nu = self.N, self.n_begin, self.n_local, self.H, self.Nu
-        p.temp, p.rew_xref = self.temp, self.rew_xref
-        p.xref_dev = vp(self.xref)
-        p.env_kind = _lib.ENV_PUSHT if self.env.kind == "pusht" else _lib.ENV_CAR2D
-        p.href = xref_len(self.env, self.xref)
-        p.Y0s_dev, p.rews_dev, p.logpd_dev = vp(self.Y0s), vp(self.rews_local), vp(self.logpd_local)
+        p.temp = self.temp
+        p.Y0s_dev, p.rews_dev, p.logpd_dev = vp(self.Y0s), vp(self.rews), vp(self.logpd)
         p.rews_all_dev, p.logpd_all_dev, p.logp_dev = vp(self.rews_all), vp(self.logpd_all), vp(self.logp_scratch)
         p.weights_dev, p.runs_dev, p.partial_dev, p.scalars_dev = vp(self.weights), vp(self.run_scratch), vp(self.partial), vp(self.scalars)
         p.P, p.rank = self.P, self.rank
+        return p
+
+    # ---- solve-level API -----------------------------------------------------------------------------------------
+    def set_step(self, i: int):
+        """device step counter <- i, of every problem (the next `step()` runs diffusion step i: reads Ybars[i], writes Ybars[i-1])"""
+        self.ctl[..., 0].fill_(int(i))
+
+    def _launch(self):
+        """the launches of one step"""
+        raise NotImplementedError
+
+    def step(self):
+        """one diffusion step at the device-resident step index (the launches, or one replay of the captured graph)"""
+        if self.graph is not None:
+            self.graph.replay()
+        else:
+            self._launch()
+
+    def capture(self):
+        """records one step in a CUDA graph; later `step()` calls replay it (parameters come from device memory)"""
+        i0 = self.ctl[..., 0].clone()
+        s = torch.cuda.Stream(device=self.device)
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            self._launch()                       # warm-up outside capture (module load, func attributes)
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        if self.P > 1:
+            import torch.distributed as dist
+            dist.barrier(group=self.group)       # every rank finished its warm-up step before anybody re-arms the counter
+        self.ctl[..., 0].copy_(i0)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self._launch()
+        self.graph = g
+        return g
+
+    def check_exchange(self):
+        """Raises if the device reported an error (`mbd_step_ctl.err`; a batch names its problems): a step ran with the step
+        counter already at 0 (one `step()` or graph replay too many; the tail kernels then write nothing), or a cross-GPU
+        rendezvous timed out (a peer died or diverged; the outputs are NaN-poisoned).  Synchronises: call it outside the step loop."""
+        err = self.ctl[..., 2].cpu().numpy().reshape(-1)
+        bad = [int(b) for b in np.nonzero(err)[0]]
+        if not bad:
+            return
+        who = "" if self.B is None else f"problems {bad}: "
+        if all(int(err[b]) == 2 for b in bad):
+            raise ops.MbdError(f"{who}the step counter ran past step 1 (a step was launched after the last one of the solve); "
+                               "that step wrote nothing")
+        if self.B is None:
+            raise ops.MbdError("cross-GPU rendezvous timed out (a peer rank stopped participating); outputs are NaN")
+        raise ops.MbdError(f"{who}device error codes {[int(err[b]) for b in bad]}")
+
+    def solve(self, log=None, log_every: int = 10, desc: Optional[str] = None):
+        """Runs a loaded solve: steps Nd - 1 ... 1, one step captured in a CUDA graph and replayed (launched directly under
+        MBD_GRAPH=0), then `check_exchange`.  log(i) runs after step i at every log_every-th step and after step 1.  desc: a tqdm
+        progress bar with this description, whose postfix is what log returns (without tqdm there is no bar and no log)."""
+        self.set_step(self.Nd - 1)
+        if os.environ.get("MBD_GRAPH", "1") != "0":
+            self.capture()
+        steps = range(self.Nd - 1, 0, -1)
+        bar = tqdm(steps, desc=desc) if desc is not None and tqdm is not None else None
+        if desc is not None and bar is None:
+            log = None
+        for n_done, i in enumerate(steps if bar is None else bar):
+            self.step()
+            if log is not None and (n_done % log_every == log_every - 1 or i == 1):
+                post = log(i)
+                if bar is not None:
+                    bar.set_postfix(post)
+        self.check_exchange()
+
+
+class DiffusionEngine(StepEngine):
+    def __init__(self, env, Nsample: int, Hsample: int, temp_sample: float, enable_demo: bool, state_init,
+                 device: Optional[torch.device] = None, group=None, Ndiffuse: int = 2, emulate=None,
+                 inputs: Optional[LaunchInputs] = None, nu: Optional[int] = None):
+        """emulate = (P, rank, bufs): rank `rank` of P ranks that all live on THIS device and exchange through the plain
+        device buffers `bufs` (one per rank) — the same kernels, flags and peer loads as a real sharded run, used by the
+        single-GPU tests (`make_emulated_ranks`).
+        env None: an engine of action size nu whose launch (1) reads `inputs` instead of an env's (LaunchInputs.none() for one
+        that drives launches 2 and 3 on constructed inputs); state_init is then unused."""
+        d = _device(device)
+        N, H = int(Nsample), int(Hsample)
+        if env is not None:
+            inputs, nu = LaunchInputs.of_env(env, state_init, enable_demo, d), env.action_size
+        self.plan = ShardPlan.from_env(N, group) if emulate is None else ShardPlan(N, emulate[0], emulate[1], None)
+        self.group, self.P, self.rank = group, self.plan.P, self.plan.rank
+        nl, HNu = self.plan.n_local, H * nu
+        # ---- exchange: P > 1 needs ONE peer-mapped symmetric buffer per rank, [rews n_local | logpd n_local | partial HNu |
+        #      2 flag rows of 8 words]; the tail kernels read the peers' slices over NVLink themselves.
+        self.sym, self.peer_ptrs = None, None
+        self.exchange = "none" if self.P == 1 else "p2p"
+        self.off_rews, self.off_logpd, self.off_partial = 0, nl, 2 * nl
+        self.off_flags = 2 * nl + HNu
+        if self.P > 1 and emulate is not None:
+            self.exchange = "p2p-emulated"
+            self.sym = emulate[2][self.rank]
+            assert self.sym.numel() == 2 * nl + HNu + 16 and self.sym.device == d
+            self.peer_ptrs = (ctypes.c_uint64 * self.P)(*[int(b.data_ptr()) for b in emulate[2]])
+        elif self.P > 1:
+            import torch.distributed as dist
+            import torch.distributed._symmetric_memory as symm_mem
+            self.sym = symm_mem.empty(2 * nl + HNu + 16, dtype=torch.float32, device=d)
+            self.sym.zero_()
+            self.sym_hdl = symm_mem.rendezvous(self.sym, dist.group.WORLD if group is None else group)
+            self.peer_ptrs = (ctypes.c_uint64 * self.P)(*[int(p) for p in self.sym_hdl.buffer_ptrs])
+            torch.cuda.synchronize()
+            dist.barrier(group=group)
+        exchange = None
+        if self.P > 1:
+            logpd = self.sym[self.off_logpd:self.off_logpd + nl] if enable_demo else None
+            exchange = (self.sym[self.off_rews:self.off_rews + nl], logpd, self.sym[self.off_partial:self.off_partial + HNu])
+        super().__init__(inputs, N, H, nu, max(int(Ndiffuse), 2), enable_demo, temp=temp_sample, device=d,
+                         n_begin=self.plan.n_begin, n_local=nl, exchange=exchange)
+        self.rews_local, self.logpd_local = self.rews, self.logpd   # this rank's samples
+
+    def _make_plan(self) -> "_lib.StepPlan":
+        p = super()._make_plan()
         if self.peer_ptrs is not None:
             p.peer_base_ptrs = ctypes.cast(self.peer_ptrs, ctypes.POINTER(ctypes.c_uint64))
         p.off_rews_words, p.off_logpd_words, p.off_partial_words, p.off_flags_words = self.off_rews, self.off_logpd, self.off_partial, self.off_flags
         p.timeout_cycles = int(float(os.environ.get("MBD_XCHG_TIMEOUT_S", "20")) * 2.0e9)
         return p
 
-    # ---- solve-level API -----------------------------------------------------------------------------------------
+    def _launch(self):
+        ops.step_launch(self._plan_c)
+
     def load_schedule(self, keys: np.ndarray, sigmas: np.ndarray, alphas: np.ndarray, alphas_bar: np.ndarray):
         """uploads the per-step parameters of a whole solve: row i = {Y0s_rng of step i, sigmas[i], update_coef(i)}"""
         Nd = self.Nd
@@ -239,57 +371,17 @@ class DiffusionEngine:
             raise ops.MbdError(f"schedule of {len(sigmas)} steps does not match the engine (Ndiffuse={Nd})")
         self.params.copy_(torch.from_numpy(pack_step_params(keys, sigmas, alphas, alphas_bar)))
 
-    def set_step(self, i: int):
-        """device step counter <- i (the next `step()` runs diffusion step i: reads Ybars[i], writes Ybars[i-1])"""
-        self.ctl[0:1].fill_(int(i))
-
-    def step(self):
-        """one diffusion step at the device-resident step index (three launches, or one replay of the captured graph)"""
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            ops.step_launch(self._plan_c)
-
-    def capture(self):
-        """records one step in a CUDA graph; later `step()` calls replay it (parameters come from device memory)"""
-        i0 = int(self.ctl[0].item())
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            ops.step_launch(self._plan_c)        # warm-up outside capture (module load, func attributes)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        if self.P > 1:
-            import torch.distributed as dist
-            dist.barrier(group=self.group)       # every rank finished its warm-up step before anybody re-arms the counter
-        self.set_step(i0)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            ops.step_launch(self._plan_c)
-        self.graph = g
-        return g
-
-    def check_exchange(self):
-        """Raises if the device reported an error (`mbd_step_ctl.err`): a cross-GPU rendezvous timed out (a peer died or
-        diverged; the outputs are NaN-poisoned), or a step ran with the step counter already at 0 (one `step()` or graph
-        replay too many; the tail kernels then write nothing).  Synchronises: call it outside the step loop."""
-        err = int(self.ctl[2].item())
-        if err == 2:
-            raise ops.MbdError("the step counter ran past step 1 (a step was launched after the last one of the solve); "
-                               "that step wrote nothing")
-        if err != 0:
-            raise ops.MbdError("cross-GPU rendezvous timed out (a peer rank stopped participating); outputs are NaN")
-
     @classmethod
-    def make_emulated_ranks(cls, env, Nsample, Hsample, temp_sample, enable_demo, state_init, P: int, Ndiffuse: int = 2, device=None):
+    def make_emulated_ranks(cls, env, Nsample, Hsample, temp_sample, enable_demo, state_init, P: int, Ndiffuse: int = 2, device=None,
+                            inputs: Optional[LaunchInputs] = None, nu: Optional[int] = None):
         """P engines = P ranks on ONE device, each with its own stream, exchanging through plain device buffers with the very
-        kernels, flags and peer loads of a real sharded run.  Drive them with `step_emulated_ranks`."""
-        d = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        HNu = int(Hsample) * env.action_size
+        kernels, flags and peer loads of a real sharded run.  Drive them with `step_emulated_ranks`.  env None: see __init__."""
+        d = _device(device)
+        HNu = int(Hsample) * (env.action_size if env is not None else nu)
         n_local = int(Nsample) // P
         bufs = [torch.zeros(2 * n_local + HNu + 16, device=d) for _ in range(P)]
-        engines = [cls(env, Nsample, Hsample, temp_sample, enable_demo, state_init, device=d, Ndiffuse=Ndiffuse, emulate=(P, r, bufs))
-                   for r in range(P)]
+        engines = [cls(env, Nsample, Hsample, temp_sample, enable_demo, state_init, device=d, Ndiffuse=Ndiffuse, emulate=(P, r, bufs),
+                       inputs=inputs, nu=nu) for r in range(P)]
         for e in engines:
             e.stream = torch.cuda.Stream(device=d)
         return engines
@@ -309,10 +401,10 @@ class DiffusionEngine:
 
     def rollout_phase(self, key, sigma: float, Ybar_i: torch.Tensor):
         """sampling + rollouts with host-side parameters (path_integral.py's update_once shares it)"""
-        if self.env.kind == "xpbd":
+        if self.model is not None:
             ops.sample_rollout(self.model, self.state_init, key, self.N, self.n_begin, self.n_local, self.H, float(sigma), Ybar_i,
                                self.Y0s, self.rews_local, xref=self.xref, logpd_out=self.logpd_local)
-        elif self.env.kind == "pusht":
+        elif self.env_kind == _lib.ENV_PUSHT:
             ops.pusht_rollout(self.params_car, self.state_init, self.Y0s.view(self.n_local, self.H, 2), key=key, n_total=self.N,
                               n_begin=self.n_begin, sigma=float(sigma), Ybar=Ybar_i, rews_out=self.rews_local)
         else:
@@ -347,7 +439,7 @@ class DiffusionEngine:
         return res, self.scalars[0]
 
 
-class BatchedDiffusionEngine:
+class BatchedDiffusionEngine(StepEngine):
     """B independent solves of one env and shape (N, H, Ndiffuse, demo) stepped in lockstep: ONE three-launch step
     (`mbd_batch_step_launch`) advances all of them.  Problem b has its own initial state, key chain, schedule (beta0 / betaT
     may differ) and temperature; every per-problem device buffer is [B, ...] with problem b's single-solve block at index b.
@@ -363,47 +455,44 @@ class BatchedDiffusionEngine:
     holds every member return of the last step.  None: today's step.
 
     ens_worst: with an ensemble, m in 1 .. K scores every sample by the mean of its m worst member returns instead of all K
-    (DESIGN.md §5m; 1 = the minimum).  0: the mean.  A captured step bakes it in, so it is fixed at construction."""
+    (DESIGN.md §5m; 1 = the minimum).  0: the mean.  A captured step bakes it in, so it is fixed at construction.
+
+    env None: an engine of action size nu whose launch (1) reads `inputs` (as in DiffusionEngine); state_inits then only count
+    the problems."""
 
     ens_factors: Optional[torch.Tensor] = None   # [B, K, 2] on the device once an ensemble is given
     ens_rews: Optional[torch.Tensor] = None      # [B, N, K]
 
     def __init__(self, env, Nsample: int, Hsample: int, temps, enable_demo: bool, state_inits, Ndiffuse: int,
                  device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None,
-                 ens_worst: int = 0):
+                 ens_worst: int = 0, inputs: Optional[LaunchInputs] = None, nu: Optional[int] = None):
         self.env = env
-        self.B = len(state_inits)
-        if self.B < 1 or len(temps) != self.B:
-            raise ValueError(f"{self.B} initial states and {len(temps)} temperatures: need one of each per problem, B >= 1")
-        ens = None if ensemble is None else ensemble_table(ensemble, self.B, env, enable_demo)
+        B = len(state_inits)
+        if B < 1 or len(temps) != B:
+            raise ValueError(f"{B} initial states and {len(temps)} temperatures: need one of each per problem, B >= 1")
+        ens = None if ensemble is None else ensemble_table(ensemble, B, env, enable_demo)
         self.ens_worst = check_ens_worst(ens_worst, None if ens is None else ens.shape[1])
-        self.N, self.H = int(Nsample), int(Hsample)
-        self.enable_demo = bool(enable_demo)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.Nu = env.action_size
-        self.HNu = self.H * self.Nu
-        self.Nd = int(Ndiffuse)
-        if self.Nd < 2:
-            raise ValueError("Ndiffuse must be at least 2")
-        per = [env_tensors(env, s, self.enable_demo, self.device) for s in state_inits]
-        self.model, self.params_car, _, self.xref = per[0]              # shared by every problem
-        self.state_init = torch.stack([p[2] for p in per]).contiguous()  # [B, state]
+        d = _device(device)
+        if env is not None:
+            inputs, nu = LaunchInputs.of_env(env, state_inits, enable_demo, d, batch=True), env.action_size
         if state_buffer is not None:
-            want = (self.B, self.state_init[0].numel())
-            if (not state_buffer.is_cuda or state_buffer.device != self.device or state_buffer.dtype != torch.float32
+            want = (B, inputs.state_init[0].numel())
+            if (not state_buffer.is_cuda or state_buffer.device != d or state_buffer.dtype != torch.float32
                     or not state_buffer.is_contiguous() or tuple(state_buffer.shape) != want):
-                raise ValueError(f"state_buffer must be a contiguous float32 tensor of shape {want} on {self.device} (got "
+                raise ValueError(f"state_buffer must be a contiguous float32 tensor of shape {want} on {d} (got "
                                  f"{state_buffer.dtype} {tuple(state_buffer.shape)} on {state_buffer.device})")
-            self.state_init = state_buffer
-        self.rew_xref = float(getattr(env, "rew_xref", 0.0))
-        self._alloc(temps)
+            inputs = dataclasses.replace(inputs, state_init=state_buffer)
         if ens is not None:
-            K = ens.shape[1]
-            self.ens_factors = torch.from_numpy(ens).to(self.device)
-            self.ens_rews = torch.empty((self.B, self.N, K), device=self.device, dtype=torch.float32)
-            p = self._plan_c
-            p.ens_factors_dev, p.ens_rews_dev, p.ens_k = self.ens_factors.data_ptr(), self.ens_rews.data_ptr(), K
+            self.ens_factors = torch.from_numpy(ens).to(d)
+            self.ens_rews = torch.empty((B, int(Nsample), ens.shape[1]), device=d, dtype=torch.float32)
+        super().__init__(inputs, Nsample, Hsample, nu, Ndiffuse, enable_demo, B=B, temps=temps, device=d)
+
+    def _make_plan(self) -> "_lib.StepPlan":
+        p = super()._make_plan()
+        if self.ens_factors is not None:
+            p.ens_factors_dev, p.ens_rews_dev, p.ens_k = self.ens_factors.data_ptr(), self.ens_rews.data_ptr(), self.ens_factors.shape[1]
             p.ens_worst = self.ens_worst
+        return p
 
     def set_ensemble(self, table):
         """rewrites the planner ensemble in place (same B and K): a captured step reads the new values on its next replay"""
@@ -413,43 +502,6 @@ class BatchedDiffusionEngine:
         if ens.shape != tuple(self.ens_factors.shape):
             raise ValueError(f"the ensemble must keep its shape {tuple(self.ens_factors.shape)} (got {ens.shape})")
         self.ens_factors.copy_(torch.from_numpy(ens))
-
-    def _alloc(self, temps):
-        """the per-problem device buffers and the C plan, from B, N, HNu, Nd, enable_demo and the env tensors set before"""
-        B, N, d = self.B, self.N, self.device
-        f = dict(device=d, dtype=torch.float32)
-        self.temps = torch.tensor(np.asarray(temps, np.float32), device=d)
-        self.Y0s = torch.empty((B, N, self.HNu), **f)
-        self.rews = torch.empty((B, N), **f)
-        self.logpd = torch.empty((B, N), **f) if self.enable_demo else None
-        self.logp_scratch = torch.empty((B, N), **f)
-        self.weights = torch.empty((B, N), **f)
-        self.scalars = torch.zeros((B, 4), **f)
-        self.run_scratch = torch.empty((B, (N + ops.RUN - 1) // ops.RUN, self.HNu), **f)
-        self.partial = torch.empty(self.HNu, **f)                       # read by sharded steps only; the plan requires it
-        self.Ybars = torch.zeros((B, self.Nd, self.HNu), **f)
-        self.rew_hist = torch.zeros((B, self.Nd), **f)
-        self.params = torch.zeros((B, self.Nd, _lib.STEP_PARAMS_WORDS), device=d, dtype=torch.int32)
-        self.ctl = torch.zeros((B, _lib.STEP_CTL_WORDS), device=d, dtype=torch.int32)
-        self.graph = None
-        self._plan_c = self._make_plan()
-
-    def _make_plan(self) -> "_lib.StepPlan":
-        p = _lib.StepPlan()
-        vp = lambda t: None if t is None else t.data_ptr()   # noqa: E731
-        p.model = self.model._h if self.model is not None else None
-        p.car_params_dev, p.state_init_dev = vp(self.params_car), vp(self.state_init)
-        p.params_dev, p.ctl_dev, p.Ybars_dev, p.rew_hist_dev = vp(self.params), vp(self.ctl), vp(self.Ybars), vp(self.rew_hist)
-        p.n_total, p.n_begin, p.n_local, p.H, p.nu = self.N, 0, self.N, self.H, self.Nu
-        p.temp, p.rew_xref = 0.0, self.rew_xref      # the per-problem temperatures come from self.temps
-        p.xref_dev = vp(self.xref)
-        p.env_kind = _lib.ENV_PUSHT if self.env.kind == "pusht" else _lib.ENV_CAR2D
-        p.href = xref_len(self.env, self.xref)
-        p.Y0s_dev, p.rews_dev, p.logpd_dev = vp(self.Y0s), vp(self.rews), vp(self.logpd)
-        p.rews_all_dev, p.logpd_all_dev, p.logp_dev = vp(self.rews), vp(self.logpd), vp(self.logp_scratch)
-        p.weights_dev, p.runs_dev, p.partial_dev, p.scalars_dev = vp(self.weights), vp(self.run_scratch), vp(self.partial), vp(self.scalars)
-        p.P, p.rank = 1, 0
-        return p
 
     # ---- solve-level API (that of DiffusionEngine, one entry per problem) -----------------------------------------------
     def load_schedule(self, keys, sigmas, alphas, alphas_bar):
@@ -462,48 +514,9 @@ class BatchedDiffusionEngine:
         tab = np.stack([pack_step_params(np.asarray(keys[b]), sigmas[b], alphas[b], alphas_bar[b]) for b in range(self.B)])
         self.params.copy_(torch.from_numpy(tab))
 
-    def set_step(self, i: int):
-        """every problem's device step counter <- i"""
-        self.ctl[:, 0].fill_(int(i))
-
-    def step(self):
-        """one diffusion step of every problem (three launches, or one replay of the captured graph)"""
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            self._launch()
-
     def _launch(self):
         """the three launches of one step of every problem"""
         ops.batch_step_launch(self._plan_c, self.B, self.Nd, self.temps)
-
-    def capture(self):
-        """records one batched step in a CUDA graph; later `step()` calls replay it"""
-        i0 = self.ctl[:, 0].clone()
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            self._launch()   # warm-up outside capture
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        self.ctl[:, 0].copy_(i0)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._launch()
-        self.graph = g
-        return g
-
-    def check_exchange(self):
-        """Raises if any problem's control block reports an error, naming the problems: err 2 = a step ran with the step
-        counter already at 0 (one `step()` or replay too many; that step wrote nothing).  Synchronises."""
-        err = self.ctl[:, 2].cpu().numpy()
-        bad = [int(b) for b in np.nonzero(err)[0]]
-        if not bad:
-            return
-        if all(int(err[b]) == 2 for b in bad):
-            raise ops.MbdError(f"problems {bad}: the step counter ran past step 1 (a step was launched after the last one of "
-                               "the solve); that step wrote nothing")
-        raise ops.MbdError(f"problems {bad}: device error codes {[int(err[b]) for b in bad]}")
 
     def problem(self, b: int):
         """the single-problem view of problem b that `final_reward` and the rollout helpers take (model, tables, state_init)"""

@@ -36,7 +36,7 @@ import torch.distributed as dist
 import mbd_b200
 from mbd_b200 import _lib, ops, prng
 from mbd_b200.planners import mbd_planner
-from mbd_b200.planners.engine import BatchedDiffusionEngine, env_tensors, key_chain, make_schedule
+from mbd_b200.planners.engine import BatchedDiffusionEngine, LaunchInputs, key_chain, make_schedule
 from mbd_b200.planners.mbd_planner import BATCH_SHARED_FIELDS, apply_recommended_params
 
 try:  # tqdm is cosmetic
@@ -254,7 +254,7 @@ class Controller:
             rng_reset, cold, warm = mpc_keys(a.seed, self.Nd, a.Nwarm, a.Nstep)
             self.host_states.append(env.reset(rng_reset))   # NOTE: rng_reset as in run_diffusion
             colds.append(cold), warms.append(warm)
-        s0 = torch.stack([env_tensors(env, s, False, d)[2].reshape(-1) for s in self.host_states]).contiguous()
+        s0 = torch.stack([LaunchInputs.of_env(env, s, False, d).state_init.reshape(-1) for s in self.host_states]).contiguous()
         self.S = s0.shape[1]
         self.venv = None
         factors = plant_factors(args_list)

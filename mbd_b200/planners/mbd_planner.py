@@ -18,12 +18,6 @@ import mbd_b200
 from mbd_b200 import ops, prng
 from mbd_b200.planners.engine import BatchedDiffusionEngine, DiffusionEngine, key_chain, make_schedule
 
-try:  # tqdm is cosmetic
-    from tqdm import tqdm
-except Exception:  # noqa: BLE001
-    tqdm = None
-
-
 ## load config
 @dataclass
 class Args:
@@ -86,26 +80,20 @@ def run_diffusion(args: Args, log_every: int = 10, return_trajectory: bool = Fal
         print(f"init sigma = {sigmas[-1]:.2e}")
 
     engine = DiffusionEngine(env, args.Nsample, args.Hsample, args.temp_sample, args.enable_demo, state_init, Ndiffuse=args.Ndiffuse)
-    HNu = args.Hsample * Nu
     # Everything the loop of mbd_planner.py:138-148 feeds into reverse_once is uploaded ONCE: the Y0s_rng chain
     # (rng, Y0s_rng = split(rng) per step, :103), sigmas[i] and the schedule scalars.  engine.Ybars row N-1 = YN = 0 and
     # row i-1 receives Ybar_{i-1}; one step is captured in a CUDA graph and replayed, nothing is copied to the host inside
     # the loop.
     rng_exp, rng = prng.split(rng)
     engine.load_schedule(key_chain(rng_exp, args.Ndiffuse), sigmas, alphas, alphas_bar)
-    engine.set_step(args.Ndiffuse - 1)
-    if os.environ.get("MBD_GRAPH", "1") != "0":
-        engine.capture()
-    steps = range(args.Ndiffuse - 1, 0, -1)
-    pbar = tqdm(steps, desc="Diffusing") if (tqdm is not None and _is_main()) else None
-    for n_done, i in enumerate(pbar if pbar is not None else steps):
-        engine.step()
-        if pbar is not None and (n_done % log_every == log_every - 1 or i == 1):
-            # the reference formats rew every step (a device->host sync each step, mbd_planner.py:147);
-            # here the sync is paid every `log_every` steps only
-            pbar.set_postfix({"rew": f"{engine.rew_hist[i].item():.2e}"})
-            engine.check_exchange()
-    engine.check_exchange()
+
+    def log(i):
+        # the reference formats rew every step (a device->host sync each step, mbd_planner.py:147);
+        # here the sync is paid every `log_every` steps only
+        rew = f"{engine.rew_hist[i].item():.2e}"
+        engine.check_exchange()
+        return {"rew": rew}
+    engine.solve(log if _is_main() else None, log_every, "Diffusing" if _is_main() else None)
     Ybars = engine.Ybars
     Yi = Ybars[: args.Ndiffuse - 1].flip(0).reshape(args.Ndiffuse - 1, args.Hsample, Nu)  # jnp.array(Ybars) order
 
@@ -178,17 +166,12 @@ def run_diffusion_batch(args_list, log_every: int = 10, return_trajectory: bool 
     engine = BatchedDiffusionEngine(env, a0.Nsample, a0.Hsample, [a.temp_sample for a in args_list], a0.enable_demo, state_inits,
                                     a0.Ndiffuse)
     engine.load_schedule(keys, [s[0] for s in scheds], [s[1] for s in scheds], [s[2] for s in scheds])
-    engine.set_step(a0.Ndiffuse - 1)
-    if os.environ.get("MBD_GRAPH", "1") != "0":
-        engine.capture()
-    steps = range(a0.Ndiffuse - 1, 0, -1)
-    pbar = tqdm(steps, desc=f"Diffusing x{engine.B}") if tqdm is not None else None
-    for n_done, i in enumerate(pbar if pbar is not None else steps):
-        engine.step()
-        if pbar is not None and (n_done % log_every == log_every - 1 or i == 1):
-            pbar.set_postfix({"rew": f"{engine.rew_hist[:, i].mean().item():.2e}"})   # mean over the problems
-            engine.check_exchange()
-    engine.check_exchange()
+
+    def log(i):
+        rew = f"{engine.rew_hist[:, i].mean().item():.2e}"   # mean over the problems
+        engine.check_exchange()
+        return {"rew": rew}
+    engine.solve(log, log_every, f"Diffusing x{engine.B}")
     Yis = [engine.Ybars[b, : a0.Ndiffuse - 1].flip(0).reshape(a0.Ndiffuse - 1, a0.Hsample, Nu) for b in range(engine.B)]
     rew_final = np.array([final_reward(env, engine.problem(b), Yis[b][-1]) for b in range(engine.B)])
     if return_trajectory:

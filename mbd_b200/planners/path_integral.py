@@ -137,15 +137,15 @@ class BatchedPathIntegralEngine(BatchedDiffusionEngine):
     capture, check_exchange, problem).  Ybars[b] holds problem b's means: row t = mu_0t of step t, row t-1 its result; launch (1)
     reads sigma_t from params[b][t].sigma.  CMA-ES writes sigma' to params[b][t-1].sigma and sigma_hist[b][t-1] on the device.
     Problem b draws the noise of a stand-alone solve with its own key and reduces in the same order, so it reproduces the B = 1
-    solve of the same inputs bit for bit.  state_buffer, ensemble and ens_worst: as in BatchedDiffusionEngine (the receding-horizon controller
-    of pi_mpc.py passes `VecEnv.state`)."""
+    solve of the same inputs bit for bit.  state_buffer, ensemble, ens_worst, inputs and nu: as in BatchedDiffusionEngine (the
+    receding-horizon controller of pi_mpc.py passes `VecEnv.state`)."""
 
     def __init__(self, env, Nsample: int, Hsample: int, temps, state_inits, Nrefine: int, update_method: str,
                  device: Optional[torch.device] = None, state_buffer: Optional[torch.Tensor] = None, ensemble=None,
-                 ens_worst: int = 0):
+                 ens_worst: int = 0, inputs=None, nu: Optional[int] = None):
         if update_method not in _lib.PI_METHODS:
             raise KeyError(update_method)
-        super().__init__(env, Nsample, Hsample, temps, False, state_inits, Nrefine, device, state_buffer, ensemble, ens_worst)
+        super().__init__(env, Nsample, Hsample, temps, False, state_inits, Nrefine, device, state_buffer, ensemble, ens_worst, inputs, nu)
         self.update_method = update_method
         self.method = _lib.PI_METHODS[update_method]
         d, f = self.device, dict(device=self.device, dtype=torch.float32)
@@ -223,17 +223,12 @@ def run_path_integral_batch(args_list, log_every: int = 10, return_trajectory: b
     eng = BatchedPathIntegralEngine(env, a0.Nsample, a0.Hsample, [a.temp_sample for a in args_list], state_inits, a0.Nrefine,
                                     a0.update_method)
     eng.load_schedule(keys)
-    eng.set_step(a0.Nrefine - 1)
-    if os.environ.get("MBD_GRAPH", "1") != "0":
-        eng.capture()
-    steps = range(a0.Nrefine - 1, 0, -1)
-    pbar = tqdm(steps, desc=f"Path Integrating x{eng.B}") if tqdm is not None else None
-    for n_done, t in enumerate(pbar if pbar is not None else steps):
-        eng.step()
-        if pbar is not None and (n_done % log_every == log_every - 1 or t == 1):
-            pbar.set_postfix({"rew": f"{eng.rew_hist[:, t].mean().item():.2e}"})   # mean over the problems
-            eng.check_exchange()
-    eng.check_exchange()
+
+    def log(t):
+        rew = f"{eng.rew_hist[:, t].mean().item():.2e}"   # mean over the problems
+        eng.check_exchange()
+        return {"rew": rew}
+    eng.solve(log, log_every, f"Path Integrating x{eng.B}")
     from mbd_b200.planners.mbd_planner import final_reward
     mu_0ts = [eng.Ybars[b, : a0.Nrefine - 1].flip(0).reshape(a0.Nrefine - 1, a0.Hsample, Nu) for b in range(eng.B)]
     rew_final = np.array([final_reward(env, eng.problem(b), mu_0ts[b][-1]) for b in range(eng.B)])

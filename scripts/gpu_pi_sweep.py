@@ -68,29 +68,20 @@ def sweep(env_name, method):
                 rew_final_sequential=[float(x) for x in seq[-1][1]], rew_final_batch=[float(x) for x in bat[-1][1]])
 
 
-class _TailEnv:
-    """car2d layout with Nu = 1 (H * Nu = any column count); tail-only launches never read it"""
-    kind = "car2d"
-    action_size = 1
-    rew_xref = 0.0
-
-    def device_params(self):
-        return torch.zeros(26, device="cuda"), torch.zeros((4, 2), device="cuda")
-
-
 def tail_ms(method, Ns, HNu=850):
-    """ms per tail (launches 2 + 3) of one problem, CUDA events over TAIL_REPS launches after 20 warm-up launches"""
+    """ms per tail (launches 2 + 3) of one problem, CUDA events over TAIL_REPS launches after 20 warm-up launches, on an engine
+    without an env (Nu = 1, H * Nu = any column count)"""
     Nd = TAIL_REPS + 22
     rng = np.random.default_rng(0)
-    x0 = np.zeros(3, np.float32)
+    none = eng.LaunchInputs.none()
     if method == "mbd":
-        e = eng.DiffusionEngine(_TailEnv(), Ns, HNu, 0.1, False, x0, Ndiffuse=Nd)
+        e = eng.DiffusionEngine(None, Ns, HNu, 0.1, False, None, Ndiffuse=Nd, inputs=none, nu=1)
         _, al, ab, sig = eng.make_schedule(1e-4, 1e-2, Nd)
         e.load_schedule(eng.key_chain(np.uint32([1, 2]), Nd), sig, al, ab)
         rews, Y = e.rews_local, e.Y0s
         launch = lambda: ops.step_tail_launch(e._plan_c)   # noqa: E731
     else:
-        e = pi.BatchedPathIntegralEngine(_TailEnv(), Ns, HNu, [0.1], [x0], Nd, method)
+        e = pi.BatchedPathIntegralEngine(None, Ns, HNu, [0.1], [None], Nd, method, inputs=none, nu=1)
         e.load_schedule([eng.key_chain(np.uint32([1, 2]), Nd)])
         rews, Y = e.rews[0], e.Y0s[0]
         launch = e.tail_step

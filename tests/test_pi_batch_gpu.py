@@ -93,20 +93,11 @@ def test_one_step_vs_oracle(orc, env_name, Nn, H, method):
 
 # ---- 2. tail-only launches on constructed returns --------------------------------------------------------------------------
 
-class _TailEnv:
-    """car2d layout with Nu = 1, so that H * Nu can be any column count; the tail never reads it"""
-    kind = "car2d"
-    action_size = 1
-    rew_xref = 0.0
-
-    def device_params(self):
-        return torch.zeros(26, device=DEV), torch.zeros((4, 2), device=DEV)
-
-
 def _tail(method, fams, Nn, HNu, temp, sigma=0.6, Y=None, mu=None):
-    """one problem per family, launches 2 and 3 of step 1 only; returns (engine, inputs)"""
+    """one problem per family, launches 2 and 3 of step 1 only, on an engine without an env (Nu = 1, so that H * Nu can be any
+    column count); returns (engine, inputs)"""
     B = len(fams)
-    e = BatchedPathIntegralEngine(_TailEnv(), Nn, HNu, [temp] * B, [np.zeros(3, f32)] * B, 2, method)
+    e = BatchedPathIntegralEngine(None, Nn, HNu, [temp] * B, [None] * B, 2, method, inputs=eng.LaunchInputs.none(), nu=1)
     e.load_schedule([np.zeros((2, 2), np.uint32)] * B)   # sigma 1 in every row; row 1 is staged below
     ins = []
     for b, fam in enumerate(fams):

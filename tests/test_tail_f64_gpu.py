@@ -28,23 +28,13 @@ TEMPS = (0.01, 0.1, 1.0, 5.0)
 BIG = f32(50.0)          # a sentinel return: every other log-weight lands below -87 at temp 0.01
 
 
-class _TailEnv:
-    """the smallest env a DiffusionEngine accepts (car2d layout, Nu = 1 so that H * Nu can be any column count); the tail
-    never reads it"""
-    kind = "car2d"
-    action_size = 1
-    rew_xref = 0.0
-
-    def device_params(self):
-        return torch.zeros(26, device=DEV), torch.zeros((4, 2), device=DEV)
-
-
 def _rig(N, HNu, P, demo=False):
-    env = _TailEnv()
-    x0 = np.zeros(3, f32)
+    """engines without an env, Nu = 1 so that H * Nu can be any column count; a demo tail needs a demonstration, of which it
+    reads nothing"""
+    inputs = eng.LaunchInputs(xref=torch.zeros((4, 2), device=DEV)) if demo else eng.LaunchInputs.none()
     if P == 1:
-        return [eng.DiffusionEngine(env, N, HNu, 0.1, demo, x0, device=DEV)]
-    return eng.DiffusionEngine.make_emulated_ranks(env, N, HNu, 0.1, demo, x0, P, device=DEV)
+        return [eng.DiffusionEngine(None, N, HNu, 0.1, demo, None, device=DEV, inputs=inputs, nu=1)]
+    return eng.DiffusionEngine.make_emulated_ranks(None, N, HNu, 0.1, demo, None, P, device=DEV, inputs=inputs, nu=1)
 
 
 def _load(engines, rews=None, Y=None, Ybar_i=None, coef=None, logpd=None):
