@@ -362,9 +362,9 @@ typedef struct mbd_vec_plan {
   float* done_dev;
   float* truncation_dev;
   float* steps_dev;
-  const float* factors_dev;     /* xpbd envs: [B][2] model factors (friction, actuator gear) of every env: env b steps with every contact
+  float* factors_dev;           /* xpbd envs: [B][2] model factors (friction, actuator gear) of every env: env b steps with every contact
                                  * friction fl(mu * F[b][0]) and every actuator gear fl(gear * F[b][1]); NULL = the nominal model.  A
-                                 * non-NULL table for car2d / pushT is MBD_EINVAL. */
+                                 * non-NULL table for car2d / pushT is MBD_EINVAL.  mbd_vec_reset_dr / mbd_vec_step_dr write it. */
 } mbd_vec_plan;
 /* env.reset(keys[b]) for every env b (keys_dev [B][2] uint32), in the threefry layout of mbd_set_prng_layout: state, first_state, obs,
  * first_obs, reward (0, pushT its reward), done, truncation 0, steps 0. */
@@ -376,6 +376,22 @@ int mbd_vec_step(const mbd_vec_plan* plan, mbd_stream s);
 int mbd_vec_set_state(const mbd_vec_plan* plan, mbd_stream s);
 /* xpbd envs: world link poses x.pos [B][L][3], x.rot [B][L][4] of the current states (PipelineEnv._make_pipeline_state) */
 int mbd_vec_world_poses(const mbd_vec_plan* plan, float* pos_dev, float* rot_dev, mbd_stream s);
+/* domain randomisation (xpbd envs; DESIGN.md §5n): a new draw of the plan's factor table at every episode of every env.
+ * keys_dev [B][2] uint32 is env b's DR key dk_b; episodes_dev [B] counts env b's episodes.  Episode e of env b steps with
+ * factors_dev[b] = (f, g): kf, kg = split(threefry2x32(dk_b, (0, e))), f = uniform(kf, (1,), flo, fhi)[0],
+ * g = uniform(kg, (1,), glo, ghi)[0], in the threefry layout of mbd_set_prng_layout.  range = {flo, fhi, glo, ghi}, finite, >= 0,
+ * lo <= hi. */
+typedef struct mbd_vec_dr {
+  const uint32_t* keys_dev;
+  int32_t* episodes_dev;
+  float range[4];
+} mbd_vec_dr;
+/* mbd_vec_reset that also zeroes episodes and writes episode 0's factors into plan->factors_dev */
+int mbd_vec_reset_dr(const mbd_vec_plan* plan, const mbd_vec_dr* dr, const uint32_t* keys_dev, mbd_stream s);
+/* mbd_vec_step that, where an env auto-resets, adds 1 to its episode count and writes that episode's factors (the step that ends an
+ * episode is computed under the old ones; launch (1) of the next step reads the new ones).  Both refuse, with MBD_EINVAL before any
+ * CUDA call, dr == NULL, car2d / pushT, a plan without factors_dev, NULL keys_dev / episodes_dev and a bad range. */
+int mbd_vec_step_dr(const mbd_vec_plan* plan, const mbd_vec_dr* dr, mbd_stream s);
 
 /* ---- PPO on the vector env (Brax's ppo.train, v0.10.x line [brax-recalled]; mbd_b200/rl) ---------------------------------------
  * The acting step, the observation statistics and GAE on the device; the nets, the loss and Adam stay in torch.  A training step's

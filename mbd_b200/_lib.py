@@ -82,6 +82,12 @@ class VecPlan(ctypes.Structure):
                 ("factors_dev", c_vp)]
 
 
+class VecDr(ctypes.Structure):
+    """mbd_vec_dr (include/mbd_b200.h): domain randomisation of a vector env's factor table"""
+    _c_name_ = "mbd_vec_dr"
+    _fields_ = [("keys_dev", c_vp), ("episodes_dev", c_vp), ("range", ctypes.c_float * 4)]
+
+
 class PpoPlan(ctypes.Structure):
     """mbd_ppo_plan (include/mbd_b200.h): the PPO acting step, observation statistics and GAE"""
     _c_name_ = "mbd_ppo_plan"
@@ -226,6 +232,8 @@ def lib():
     L.mbd_vec_step.argtypes = [ctypes.POINTER(VecPlan), c_vp]
     L.mbd_vec_set_state.argtypes = [ctypes.POINTER(VecPlan), c_vp]
     L.mbd_vec_world_poses.argtypes = [ctypes.POINTER(VecPlan), c_vp, c_vp, c_vp]
+    L.mbd_vec_reset_dr.argtypes = [ctypes.POINTER(VecPlan), ctypes.POINTER(VecDr), c_vp, c_vp]
+    L.mbd_vec_step_dr.argtypes = [ctypes.POINTER(VecPlan), ctypes.POINTER(VecDr), c_vp]
     L.mbd_ppo_act.argtypes = [ctypes.POINTER(PpoPlan), ctypes.c_int, c_vp]
     L.mbd_ppo_obs_stats.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
     L.mbd_ppo_gae.argtypes = [ctypes.POINTER(PpoPlan), c_vp]
@@ -250,7 +258,7 @@ def lib():
 
 
 EXPORTS = ["mbd_set_kernel_variant", "mbd_set_prng_layout", "mbd_model_set_warp_order", "mbd_last_error", "mbd_device_count", "mbd_model_create", "mbd_model_destroy", "mbd_sample",
-           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_ens_score", "mbd_ens_draw", "mbd_bbo_batch_step_launch", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_mpc_advance", "mbd_mpc_pi_advance", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
+           "mbd_rollout", "mbd_rollout_traj", "mbd_sample_rollout", "mbd_car2d_rollout", "mbd_pusht_rollout", "mbd_softmax_weights", "mbd_weighted_sum", "mbd_weighted_sum_runs", "mbd_weighted_sqerr_sum", "mbd_test_arith", "mbd_test_err", "mbd_test_sweep","mbd_update", "mbd_step_launch", "mbd_batch_step_launch", "mbd_pi_batch_step_launch", "mbd_ens_score", "mbd_ens_draw", "mbd_bbo_batch_step_launch", "mbd_mnist_step_launch", "mbd_mnist_forward", "mbd_mnist_batch_indices", "mbd_vec_reset", "mbd_vec_step", "mbd_vec_set_state", "mbd_vec_world_poses", "mbd_vec_reset_dr", "mbd_vec_step_dr", "mbd_ppo_act", "mbd_ppo_obs_stats", "mbd_ppo_gae", "mbd_sac_act", "mbd_sac_record", "mbd_sac_sample", "mbd_sac_learn_scratch", "mbd_sac_update", "mbd_mpc_advance", "mbd_mpc_pi_advance", "mbd_step_tail_launch", "mbd_step_launch_ev", "mbd_event_create", "mbd_event_destroy", "mbd_event_record",
            "mbd_event_sync", "mbd_event_elapsed_ms", "mbd_ffma_peak"]
 
 

@@ -93,9 +93,20 @@ __device__ __forceinline__ void vec_reset_one(const mbd_vec_plan& p, const VecDi
   mbd_k64_pipeline_init(p.kin_dev, q, qd, st);
 }
 
+// domain randomisation: the factors of episode e of env b into factors[b] (mbd_vec_dr; envs.vec.dr_factors):
+// kf, kg = split(fold_in(dk_b, e)); f = uniform(kf, (1,), flo, fhi)[0], g = uniform(kg, (1,), glo, ghi)[0]
+__device__ __forceinline__ void vec_dr_draw(const mbd_vec_plan& p, const mbd_vec_dr& dr, int b, int e, int part) {
+  uint32_t k[2], kf[2], kg[2];
+  mbd_threefry2x32(dr.keys_dev[2 * b], dr.keys_dev[2 * b + 1], 0u, (uint32_t)e, &k[0], &k[1]);   // fold_in(dk_b, e)
+  vec_split(k[0], k[1], 2, 0, part, kf);
+  vec_split(k[0], k[1], 2, 1, part, kg);
+  p.factors_dev[2 * b] = vec_uniform(kf, 0, 1, part, dr.range[0], dr.range[1]);
+  p.factors_dev[2 * b + 1] = vec_uniform(kg, 0, 1, part, dr.range[2], dr.range[3]);
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(kVecThreads) k_vec(mbd_vec_plan p, VecDims d, const uint32_t* __restrict__ keys, int part,
-                                                     float* __restrict__ wpos, float* __restrict__ wrot) {
+                                                     float* __restrict__ wpos, float* __restrict__ wrot, mbd_vec_dr dr) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= p.B) return;
   float* st = p.state_dev + (size_t)b * d.S;
@@ -123,6 +134,10 @@ __global__ void __launch_bounds__(kVecThreads) k_vec(mbd_vec_plan p, VecDims d, 
     p.done_dev[b] = done;
     p.truncation_dev[b] = 0.0f;
     p.steps_dev[b] = 0.0f;
+    if (MODE == kVecReset && dr.keys_dev) {   // episode 0
+      dr.episodes_dev[b] = 0;
+      vec_dr_draw(p, dr, b, 0, part);
+    }
     return;
   }
   // MODE == kVecStep: launch (1) left the next state in next_state and the step's reward in reward
@@ -146,6 +161,12 @@ __global__ void __launch_bounds__(kVecThreads) k_vec(mbd_vec_plan p, VecDims d, 
   for (int k = 0; k < d.S; ++k) st[k] = src[k];
   const float* fo = p.first_obs_dev + (size_t)b * d.O;
   for (int k = 0; k < d.O; ++k) ob[k] = reset ? fo[k] : o[k];
+  // the next episode's factors; launch (1) of this step has read the old ones, launch (1) of the next step reads these
+  if (reset && dr.keys_dev) {
+    const int e = dr.episodes_dev[b] + 1;
+    dr.episodes_dev[b] = e;
+    vec_dr_draw(p, dr, b, e, part);
+  }
 }
 
 }  // namespace mbd

@@ -17,6 +17,10 @@ and reward bit for bit, observations within one float32 ulp), see DESIGN.md §5e
 The xpbd envs can step every env with its own friction and actuator strength (DESIGN.md §5k):
 
     venv.set_model_factors(friction=f, gear=g)  # scalars or [B] arrays; env b is scaled_env(env, f[b], g[b])
+
+or draw new factors at every episode of every env, inside the step (domain randomisation, DESIGN.md §5n):
+
+    venv.set_domain_randomization((0.5, 1.5), (0.7, 1.3), keys)   # episode e of env b: dr_factors(keys[b], e, ...)
 """
 from __future__ import annotations
 
@@ -28,7 +32,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import _lib, ops, prng
 from ..model import blob as blob_mod
 from .ant import Ant
 from .base import PipelineEnv
@@ -159,6 +163,35 @@ def factor_column(value, B: int, name: str) -> np.ndarray:
     return f
 
 
+def dr_range(friction_range, gear_range) -> np.ndarray:
+    """mbd_vec_dr.range: float32 [flo, fhi, glo, ghi]; ValueError unless each range is a pair of finite values >= 0 with lo <= hi
+    (in float32, as the kernel reads them)"""
+    out = []
+    for name, r in (("friction_range", friction_range), ("gear_range", gear_range)):
+        try:
+            v = np.asarray(r, dtype=np.float64)
+        except (TypeError, ValueError):
+            raise ValueError(f"{name} must be a pair (lo, hi) (got {r!r})") from None
+        if v.shape != (2,):
+            raise ValueError(f"{name} must be a pair (lo, hi) (got {r!r})")
+        with np.errstate(over="ignore"):
+            f = v.astype(np.float32)
+        if not (np.isfinite(f).all() and (f >= 0).all()):
+            raise ValueError(f"{name} must be finite and >= 0 (got {v.tolist()})")
+        if f[0] > f[1]:
+            raise ValueError(f"{name} needs lo <= hi (got {v.tolist()})")
+        out += [f[0], f[1]]
+    return np.float32(out)
+
+
+def dr_factors(key, episode: int, friction_range, gear_range):
+    """(f, g): the model factors of episode `episode` of an env with DR key `key` (DESIGN.md §5n), the specification of the vector
+    env's draw: kf, kg = split(fold_in(key, episode)); f = uniform(kf, (1,), flo, fhi)[0]; g = uniform(kg, (1,), glo, ghi)[0]"""
+    r = dr_range(friction_range, gear_range)
+    kf, kg = prng.split(prng.fold_in(key, episode))
+    return prng.uniform(kf, (1,), r[0], r[1])[0], prng.uniform(kg, (1,), r[2], r[3])[0]
+
+
 def scaled_env(env: PipelineEnv, friction: float = 1.0, gear: float = 1.0) -> PipelineEnv:
     """the specification of a vector env stepped with model factors (friction, gear): a host env of the same class whose every
     contact friction is fl(mu * friction) and every actuator gear fl(gear_a * gear), in float32 as the kernel forms them, with its
@@ -225,6 +258,9 @@ class VecEnv:
             setattr(P, name + "_dev", getattr(self, name).data_ptr())
         self.plan = P
         self.factors: Optional[torch.Tensor] = None   # [B, 2] friction | gear factors once set_model_factors gave any
+        self.dr: Optional[_lib.VecDr] = None            # domain randomisation (set_domain_randomization): the mbd_vec_dr
+        self.dr_keys: Optional[torch.Tensor] = None   # [B, 2] DR keys and [B] episode counts it points to
+        self.dr_episodes: Optional[torch.Tensor] = None
 
     def set_model_factors(self, friction=None, gear=None) -> None:
         """step env b with every contact friction scaled by friction[b] and every actuator gear by gear[b] (xpbd envs): env b then
@@ -236,13 +272,47 @@ class VecEnv:
         B = self.num_envs
         fr = factor_column(1.0 if friction is None else friction, B, "friction")
         gr = factor_column(1.0 if gear is None else gear, B, "gear")
+        self.dr = None   # fixed factors end domain randomisation
         if friction is None and gear is None:
             self.plan.factors_dev = None
             return
-        if self.factors is None:
-            self.factors = torch.empty((B, 2), device=self.device, dtype=torch.float32)
+        self._factor_table()
         self.factors.copy_(torch.from_numpy(np.stack([fr, gr], axis=1)))
+
+    def set_domain_randomization(self, friction_range, gear_range, keys) -> None:
+        """domain randomisation (xpbd envs, DESIGN.md §5n): every episode of env b steps with factors drawn from its DR key keys[b]
+        and its episode count, (f, g) = dr_factors(keys[b], e, friction_range, gear_range); env b in episode e steps as the nominal
+        VecEnv of scaled_env(env, f, g), bit for bit.  keys: uint32 [B, 2] (numpy or cuda, as in reset).  It takes effect at the next
+        reset, which zeroes the episode counts and writes episode 0's factors; each auto-reset draws the next episode's.  `factors`
+        holds the current table and `dr_episodes` the counts.  reset / step then launch mbd_vec_reset_dr / mbd_vec_step_dr with
+        `dr`; code that launches ops.vec_step itself passes `venv.dr`.  set_model_factors ends it."""
+        if self.spec.kind != _lib.VEC_XPBD:
+            raise ValueError("domain randomisation exists for the positional (xpbd) envs only")
+        r = dr_range(friction_range, gear_range)
+        k = self._key_bits(keys).clone()   # owned: a later write to the caller's tensor does not change the draws
+        self._factor_table()
+        if self.dr_episodes is None:
+            self.dr_episodes = torch.zeros(self.num_envs, device=self.device, dtype=torch.int32)
+        self.dr_keys = k
+        dr = _lib.VecDr()
+        dr.keys_dev, dr.episodes_dev = k.data_ptr(), self.dr_episodes.data_ptr()
+        dr.range[:] = [float(x) for x in r]
+        self.dr = dr
+
+    def _factor_table(self):
+        """the [B, 2] factor table (allocated once, 1 everywhere) and the plan's pointer to it"""
+        if self.factors is None:
+            self.factors = torch.ones((self.num_envs, 2), device=self.device, dtype=torch.float32)
         self.plan.factors_dev = self.factors.data_ptr()
+
+    def _key_bits(self, keys) -> torch.Tensor:
+        """uint32 [B, 2] keys (numpy, or a cuda tensor of uint32 / int32 bits) as an int32 device tensor; the shape is checked first"""
+        shape = tuple(keys.shape) if isinstance(keys, torch.Tensor) else np.shape(keys)
+        if shape != (self.num_envs, 2) or (isinstance(keys, torch.Tensor) and keys.dtype not in (torch.uint32, torch.int32)):
+            raise ValueError(f"keys must be uint32 [{self.num_envs}, 2]")
+        if isinstance(keys, torch.Tensor):
+            return keys.to(self.device).contiguous().view(torch.int32)
+        return torch.as_tensor(np.ascontiguousarray(keys, dtype=np.uint32).view(np.int32), device=self.device)
 
     # ---- the batched env API -------------------------------------------------------------------------------------------------
     def _view(self) -> VecState:
@@ -251,15 +321,9 @@ class VecEnv:
 
     def reset(self, keys) -> VecState:
         """vmap(env.reset)(keys): keys uint32 [B, 2] (numpy, or a cuda tensor of uint32 / int32 bits)"""
-        if isinstance(keys, torch.Tensor):
-            k = keys.to(self.device).contiguous()
-            k = k.view(torch.int32) if k.dtype in (torch.uint32, torch.int32) else None
-        else:
-            k = torch.as_tensor(np.ascontiguousarray(keys, dtype=np.uint32).view(np.int32), device=self.device)
-        if k is None or tuple(k.shape) != (self.num_envs, 2):
-            raise ValueError(f"keys must be uint32 [{self.num_envs}, 2]")
+        k = self._key_bits(keys)
         with torch.cuda.device(self.device):
-            ops.vec_reset(self.plan, k)
+            ops.vec_reset(self.plan, k, self.dr)
         return self._view()
 
     def step(self, actions: Optional[torch.Tensor] = None) -> VecState:
@@ -268,7 +332,7 @@ class VecEnv:
         if actions is not None and actions.data_ptr() != self.actions.data_ptr():
             self.actions.copy_(actions)
         with torch.cuda.device(self.device):
-            ops.vec_step(self.plan)
+            ops.vec_step(self.plan, self.dr)
         return self._view()
 
     def set_state(self, raw) -> VecState:

@@ -238,14 +238,23 @@ def mnist_batch_indices(sub_keys: np.ndarray, Ndiffuse: int, n_data: int, N: int
     torch.cuda.current_stream().synchronize()   # the scratch is freed on return
 
 
-def vec_reset(plan: "_lib.VecPlan", keys: torch.Tensor):
-    """env.reset(keys[b]) of every env of a vector-env plan (mbd_vec_reset); keys [B, 2] int32 / uint32 bits on the device"""
-    check(_lib.lib().mbd_vec_reset(ctypes.byref(plan), _p(_dev(keys, torch.int32)), _stream()), "mbd_vec_reset")
+def vec_reset(plan: "_lib.VecPlan", keys: torch.Tensor, dr: "Optional[_lib.VecDr]" = None):
+    """env.reset(keys[b]) of every env of a vector-env plan (mbd_vec_reset); keys [B, 2] int32 / uint32 bits on the device.  With
+    domain randomisation `dr`: mbd_vec_reset_dr (also episode 0's factors)."""
+    k = _p(_dev(keys, torch.int32))
+    if dr is None:
+        check(_lib.lib().mbd_vec_reset(ctypes.byref(plan), k, _stream()), "mbd_vec_reset")
+    else:
+        check(_lib.lib().mbd_vec_reset_dr(ctypes.byref(plan), ctypes.byref(dr), k, _stream()), "mbd_vec_reset_dr")
 
 
-def vec_step(plan: "_lib.VecPlan"):
-    """one env step of every env with the actions in the plan's buffer (mbd_vec_step: two launches, graph-capturable)"""
-    check(_lib.lib().mbd_vec_step(ctypes.byref(plan), _stream()), "mbd_vec_step")
+def vec_step(plan: "_lib.VecPlan", dr: "Optional[_lib.VecDr]" = None):
+    """one env step of every env with the actions in the plan's buffer (mbd_vec_step: two launches, graph-capturable).  With domain
+    randomisation `dr`: mbd_vec_step_dr (also each auto-reset's new factors)."""
+    if dr is None:
+        check(_lib.lib().mbd_vec_step(ctypes.byref(plan), _stream()), "mbd_vec_step")
+    else:
+        check(_lib.lib().mbd_vec_step_dr(ctypes.byref(plan), ctypes.byref(dr), _stream()), "mbd_vec_step_dr")
 
 
 def vec_set_state(plan: "_lib.VecPlan"):

@@ -95,6 +95,11 @@ def _threefry_int(k0: int, k1: int, c0: int, c1: int):
     return x0, x1
 
 
+def fold_in(key, data: int) -> np.ndarray:
+    """jax.random.fold_in(key, data) **[jax-recalled]**: threefry2x32(key, (0, data))"""
+    return np.array(_threefry_int(int(key[0]), int(key[1]), 0, int(data) & 0xFFFFFFFF), np.uint32)
+
+
 def split2(key):
     """split(key, 2) for the planner's `rng, Y0s_rng = split(rng)` chain: returns (new_key, sub_key) as uint32[2] arrays"""
     k0, k1 = int(key[0]), int(key[1])

@@ -24,7 +24,9 @@ import torch
 
 from .. import _lib, ops, prng
 from ..envs import get_env
-from ..envs.vec import VecEnv
+from ..envs.base import PipelineEnv
+from ..envs.vec import VecEnv, dr_range
+from ..prng import fold_in
 from . import networks as nets
 
 
@@ -45,9 +47,25 @@ def counts(num_timesteps: int, num_envs: int, batch_size: int, num_minibatches: 
     return Counts(batch_size * num_minibatches // num_envs, per_step, after, int(math.ceil(num_timesteps / (after * per_step))))
 
 
-def fold_in(key, data: int) -> np.ndarray:
-    """jax.random.fold_in(key, data) **[jax-recalled]**: threefry2x32(key, (0, data))"""
-    return np.array(prng._threefry_int(int(key[0]), int(key[1]), 0, int(data) & 0xFFFFFFFF), np.uint32)
+def dr_keys(seed: int, num_envs: int) -> np.ndarray:
+    """[num_envs, 2] the DR keys of the training envs (DESIGN.md §5n): split(PRNGKey(2^33 | seed), num_envs).  The root [2, seed]
+    differs from the trainer's [0, seed] and from the controllers' member keys [1, seed], so no chain shares a key with them."""
+    if not 0 <= int(seed) < 1 << 32:
+        raise ValueError(f"domain randomisation needs a seed in 0 .. 2^32 - 1 (got {seed})")
+    return prng.split(prng.PRNGKey((2 << 32) | int(seed)), num_envs)
+
+
+def check_randomization(randomization: Optional[dict], env) -> Optional[tuple]:
+    """the trainers' `randomization` argument checked on the host: None, or dict(friction_range=(lo, hi), gear_range=(lo, hi)) on an
+    xpbd env (either range may be omitted: (1, 1)).  Returns None or (friction_range, gear_range) as float32 pairs."""
+    if randomization is None:
+        return None
+    if not isinstance(randomization, dict) or set(randomization) - {"friction_range", "gear_range"}:
+        raise ValueError(f"randomization must be None or dict(friction_range=(lo, hi), gear_range=(lo, hi)) (got {randomization!r})")
+    if not isinstance(env, PipelineEnv):
+        raise ValueError(f"domain randomisation exists for the positional (xpbd) envs only, not {type(env).__name__}")
+    r = dr_range(randomization.get("friction_range", (1.0, 1.0)), randomization.get("gear_range", (1.0, 1.0)))
+    return (r[0], r[1]), (r[2], r[3])
 
 
 @dataclasses.dataclass
@@ -168,7 +186,8 @@ class PPOTrainer:
     def __init__(self, env, num_timesteps: int, episode_length: int, num_envs: int, num_eval_envs: int, learning_rate: float,
                  entropy_cost: float, discounting: float, seed: int, unroll_length: int, batch_size: int, num_minibatches: int,
                  num_updates_per_batch: int, num_evals: int, normalize_observations: bool, reward_scaling: float,
-                 clipping_epsilon: float, gae_lambda: float, device=None):
+                 clipping_epsilon: float, gae_lambda: float, device=None, randomization: Optional[dict] = None):
+        self.dr = check_randomization(randomization, env)
         _lib.require_gpu()
         if batch_size > _lib.PPO_MAX_MB:
             raise ValueError(f"batch_size (trajectories per minibatch) must be at most {_lib.PPO_MAX_MB}")
@@ -178,6 +197,7 @@ class PPOTrainer:
         self.episode_length, self.entropy_cost, self.clip = episode_length, entropy_cost, clipping_epsilon
         self.normalize_observations = normalize_observations
         self.keys = key_chain(seed, c, num_envs, unroll_length, num_updates_per_batch, num_minibatches, num_eval_envs, episode_length)
+        self.dr_keys = dr_keys(seed, num_envs) if self.dr is not None else None
         with torch.cuda.device(d):
             self._setup(num_eval_envs, learning_rate, discounting, reward_scaling, gae_lambda)
 
@@ -237,6 +257,8 @@ class PPOTrainer:
         self.eval_keys = _i32(K.eval_act.reshape(-1, 2), d)
         self.eval_reset = _i32(K.eval_reset, d)
         self.actor = Actor(self.evenv, self.theta.detach()[:self.Np], self.mean, self.std, self.eval_keys)
+        if self.dr is not None:          # the training envs only: evaluation stays on the nominal model
+            self.venv.set_domain_randomization(*self.dr, self.dr_keys)
         self.venv.reset(_i32(K.env, d))
         self.step_index = 0
         self.eval_index = 0
@@ -247,7 +269,7 @@ class PPOTrainer:
         """T x (act, env step): one of Brax's generate_unroll calls"""
         for _ in range(self.T):
             ops.ppo_act(self.plan, _lib.PPO_ACT)
-            ops.vec_step(self.venv.plan)
+            ops.vec_step(self.venv.plan, self.venv.dr)
 
     def sgd_step(self):
         """one minibatch: gather (outside autograd), forward, GAE, loss, backward, Adam"""
@@ -365,10 +387,11 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
           num_minibatches: int = 16, num_updates_per_batch: int = 2, num_evals: int = 1, num_resets_per_eval: int = 0,
           normalize_observations: bool = False, reward_scaling: float = 1.0, clipping_epsilon: float = 0.3, gae_lambda: float = 0.95,
           deterministic_eval: bool = False, normalize_advantage: bool = True,
-          progress_fn: Callable[[int, dict], None] = lambda *a: None, capture: bool = True):
+          progress_fn: Callable[[int, dict], None] = lambda *a: None, capture: bool = True, randomization: Optional[dict] = None):
     """ppo.train with Brax's signature and defaults for the arguments the reference passes.  Returns (make_inference_fn, params,
     metrics): make_inference_fn(params) gives an `Actor` factory for a VecEnv; params is a dict of numpy arrays (policy, value, the
-    observation statistics)."""
+    observation statistics).  randomization = dict(friction_range=(lo, hi), gear_range=(lo, hi)) trains with domain randomisation
+    (DESIGN.md §5n): every episode of every training env draws its own model factors; the evaluation envs stay nominal."""
     if action_repeat != 1:
         raise NotImplementedError("action_repeat != 1 is not built (the vector env steps once per action)")
     if num_resets_per_eval != 0:
@@ -378,7 +401,7 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
     env = get_env(environment) if isinstance(environment, str) else environment
     tr = PPOTrainer(env, num_timesteps, episode_length, num_envs, num_eval_envs, learning_rate, entropy_cost, discounting, seed,
                     unroll_length, batch_size, num_minibatches, num_updates_per_batch, num_evals, normalize_observations,
-                    reward_scaling, clipping_epsilon, gae_lambda)
+                    reward_scaling, clipping_epsilon, gae_lambda, randomization=randomization)
     if capture:
         tr.capture()
     c = tr.c

@@ -26,8 +26,9 @@ import torch.nn.functional as F
 from .. import _lib, ops, prng
 from ..envs import get_env
 from ..envs.vec import VecEnv
+from ..prng import fold_in
 from . import networks as nets
-from .ppo import _i32, fold_in
+from .ppo import _i32, check_randomization, dr_keys
 
 ALPHA_LEARNING_RATE = 3e-4      # Brax's alpha optimiser is adam(3e-4) whatever learning_rate is
 
@@ -304,9 +305,10 @@ class SACTrainer:
     def __init__(self, env, num_timesteps: int, episode_length: int, num_envs: int, num_eval_envs: int, learning_rate: float,
                  discounting: float, seed: int, batch_size: int, num_evals: int, normalize_observations: bool, reward_scaling: float,
                  tau: float, min_replay_size: int, max_replay_size: int, grad_updates_per_step: int, device=None,
-                 learner: str = "torch"):
+                 learner: str = "torch", randomization: Optional[dict] = None):
         if learner not in LEARNERS:
             raise ValueError(f"learner must be one of {LEARNERS}, not {learner!r}")
+        self.dr = check_randomization(randomization, env)
         self.learner_kind = learner
         _lib.require_gpu()
         if not num_envs <= max_replay_size <= _lib.SAC_MAX_CAPACITY:
@@ -316,6 +318,7 @@ class SACTrainer:
         self.env, self.B, self.mb, self.G, self.cap = env, num_envs, batch_size, grad_updates_per_step, max_replay_size
         self.episode_length, self.normalize_observations = episode_length, normalize_observations
         self.keys = key_chain(seed, c, num_envs, grad_updates_per_step, num_eval_envs, episode_length)
+        self.dr_keys = dr_keys(seed, num_envs) if self.dr is not None else None
         with torch.cuda.device(d):
             self._setup(num_eval_envs, learning_rate, discounting, reward_scaling, tau)
 
@@ -372,6 +375,8 @@ class SACTrainer:
         self.eval_keys = _i32(K.eval_act.reshape(-1, 2), d)
         self.eval_reset = _i32(K.eval_reset, d)
         self.actor = Actor(self.evenv, self.learner.policy.detach(), self.mean, self.std, self.eval_keys)
+        if self.dr is not None:          # the training envs only: evaluation stays on the nominal model
+            self.venv.set_domain_randomization(*self.dr, self.dr_keys)
         self.venv.reset(_i32(K.env, d))
         self.step_index = 0
         self.eval_index = 0
@@ -381,7 +386,7 @@ class SACTrainer:
     def actor_step(self):
         """acting.actor_step + running_statistics.update + insert: act, env step, record, statistics"""
         ops.sac_act(self.plan, _lib.SAC_ACT)
-        ops.vec_step(self.venv.plan)
+        ops.vec_step(self.venv.plan, self.venv.dr)
         ops.sac_record(self.plan)
         if self.normalize_observations:
             ops.ppo_obs_stats(self.stat_plan)
@@ -496,11 +501,12 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
           normalize_observations: bool = False, max_devices_per_host: Optional[int] = None, reward_scaling: float = 1.0,
           tau: float = 0.005, min_replay_size: int = 0, max_replay_size: Optional[int] = None, grad_updates_per_step: int = 1,
           deterministic_eval: bool = False, progress_fn: Callable[[int, dict], None] = lambda *a: None, capture: bool = True,
-          learner: str = "torch"):
+          learner: str = "torch", randomization: Optional[dict] = None):
     """sac.train with Brax's signature and defaults for the arguments the reference passes.  Returns (make_inference_fn, params,
     metrics): make_inference_fn(params) gives an `Actor` factory for a VecEnv; params is a dict of numpy arrays (policy, q, target_q,
     log_alpha, the observation statistics).  One device: max_devices_per_host is accepted and has nothing to choose.  learner:
-    "torch" (`Learner`, the default) or "fused" (`FusedLearner`, the update as two CUDA launches)."""
+    "torch" (`Learner`, the default) or "fused" (`FusedLearner`, the update as two CUDA launches).  randomization: as ppo.train's
+    (domain randomisation of the training envs, DESIGN.md §5n)."""
     if learner not in LEARNERS:
         raise ValueError(f"learner must be one of {LEARNERS}, not {learner!r}")
     if action_repeat != 1:
@@ -512,7 +518,7 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
     env = get_env(environment) if isinstance(environment, str) else environment
     tr = SACTrainer(env, num_timesteps, episode_length, num_envs, num_eval_envs, learning_rate, discounting, seed, batch_size, num_evals,
                     normalize_observations, reward_scaling, tau, min_replay_size, max_replay_size, grad_updates_per_step,
-                    learner=learner)
+                    learner=learner, randomization=randomization)
     if capture:
         tr.capture()
     c = tr.c

@@ -3,7 +3,9 @@
 Trains PPO (mbd_b200.rl.ppo) with the reference's per-env hyperparameters, prints `step: N, episode return: X` at every evaluation,
 `time to jit`, `time to train`, saves the parameters to results/{env}/params.npz (Brax's pickle format is not reproduced), runs the
 reference's final evaluation (8 episodes of 50 steps, 40 for pushT, one env, the reference's key chain) and writes results/{env}/RL.html.
-Extensions: --num_timesteps and --seed override the table for short runs.  hopper, which the reference trains with SAC, has its own
+Extensions: --num_timesteps and --seed override the table for short runs; --dr_friction lo hi / --dr_gear lo hi train with domain
+randomisation (DESIGN.md §5n: every episode of every training env draws its friction and actuator-gear factors from those ranges, an
+omitted one is 1 1; evaluation stays on the nominal model) and write params_dr.npz / RL_dr.html instead.  hopper, which the reference trains with SAC, has its own
 script (python -m mbd_b200.rl.train_sac --env_name hopper); pusher fails in get_env as in the reference.  ant trains without Brax's
 unhealthy termination: the host Ant and the vector env never terminate.
 """
@@ -36,12 +38,31 @@ def ppo_config(env_name: str) -> dict:
     return cfg
 
 
-def main(argv=None):
+def add_dr_flags(ap: argparse.ArgumentParser) -> None:
+    ap.add_argument("--dr_friction", type=float, nargs=2, default=None, metavar=("LO", "HI"),
+                    help="domain randomisation: the range of every training episode's friction factor")
+    ap.add_argument("--dr_gear", type=float, nargs=2, default=None, metavar=("LO", "HI"),
+                    help="domain randomisation: the range of every training episode's actuator-gear factor")
+
+
+def randomization(a: argparse.Namespace):
+    """the trainers' `randomization` from --dr_friction / --dr_gear (None without either; an omitted one is (1, 1))"""
+    if a.dr_friction is None and a.dr_gear is None:
+        return None
+    return dict(friction_range=tuple(a.dr_friction or (1.0, 1.0)), gear_range=tuple(a.dr_gear or (1.0, 1.0)))
+
+
+def parse_args(argv=None) -> argparse.Namespace:
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--env_name", default="halfcheetah")
     ap.add_argument("--num_timesteps", type=int, default=None, help="override the table's num_timesteps")
     ap.add_argument("--seed", type=int, default=None, help="override the table's seed")
-    a = ap.parse_args(argv)
+    add_dr_flags(ap)
+    return ap.parse_args(argv)
+
+
+def main(argv=None):
+    a = parse_args(argv)
     if a.env_name in SAC_ENVS:
         raise SystemExit(f"{a.env_name}: the reference trains it with Brax SAC, not PPO: run python -m mbd_b200.rl.train_sac --env_name {a.env_name}")
 
@@ -56,9 +77,11 @@ def main(argv=None):
         cfg["num_timesteps"] = a.num_timesteps
     if a.seed is not None:
         cfg["seed"] = a.seed
+    dr = randomization(a)
+    ppo.check_randomization(dr, env)
     progress, times = progress_printer()
-    make_inference_fn, params, _ = ppo.train(environment=env, progress_fn=progress, **cfg)
-    post_training(a.env_name, env, make_inference_fn, params, times)
+    make_inference_fn, params, _ = ppo.train(environment=env, progress_fn=progress, randomization=dr, **cfg)
+    post_training(a.env_name, env, make_inference_fn, params, times, tag="_dr" if dr else "")
 
 
 def progress_printer():
@@ -73,9 +96,10 @@ def progress_printer():
     return progress, times
 
 
-def post_training(env_name, env, make_inference_fn, params, times):
-    """the reference script's tail after training: the times, results/{env}/params.npz, the mean reward of 8 episodes of 50 steps
-    (40 for pushT) on one env with the reference's key chain, and results/{env}/RL.html of one more rollout"""
+def post_training(env_name, env, make_inference_fn, params, times, tag: str = ""):
+    """the reference script's tail after training: the times, results/{env}/params{tag}.npz, the mean reward of 8 episodes of 50
+    steps (40 for pushT) on one env of the nominal model with the reference's key chain, and results/{env}/RL{tag}.html of one more
+    rollout"""
     import torch
 
     import mbd_b200
@@ -90,7 +114,7 @@ def post_training(env_name, env, make_inference_fn, params, times):
 
     path = f"{mbd_b200.__path__[0]}/../results/{env_name}"
     os.makedirs(path, exist_ok=True)
-    np.savez(f"{path}/params.npz", **params)
+    np.savez(f"{path}/params{tag}.npz", **params)
 
     venv = VecEnv(env, 1)
     actor = make_inference_fn(params)(venv)
@@ -117,7 +141,7 @@ def post_training(env_name, env, make_inference_fn, params, times):
         actor.act(act_rng)
         venv.step()
     torch.cuda.synchronize()
-    with open(f"{path}/RL.html", "w") as f:
+    with open(f"{path}/RL{tag}.html", "w") as f:
         f.write(brax_json.render(env.sys, rollout, env.dt))
 
 
