@@ -16,7 +16,6 @@ from __future__ import annotations
 import ctypes
 import dataclasses
 import math
-import time
 from typing import Callable, Optional
 
 import numpy as np
@@ -24,10 +23,10 @@ import torch
 
 from .. import _lib, ops, prng
 from ..envs import get_env
-from ..envs.base import PipelineEnv
-from ..envs.vec import VecEnv, dr_range
 from ..prng import fold_in
+from . import common
 from . import networks as nets
+from .common import _i32, check_randomization, dr_keys  # noqa: F401  (ppo.check_randomization and ppo.dr_keys are public)
 
 
 # ---- step accounting and the key chain (host only) -------------------------------------------------------------------------------
@@ -45,27 +44,6 @@ def counts(num_timesteps: int, num_envs: int, batch_size: int, num_minibatches: 
     per_step = batch_size * num_minibatches * unroll_length
     after = max(num_evals - 1, 1)
     return Counts(batch_size * num_minibatches // num_envs, per_step, after, int(math.ceil(num_timesteps / (after * per_step))))
-
-
-def dr_keys(seed: int, num_envs: int) -> np.ndarray:
-    """[num_envs, 2] the DR keys of the training envs (DESIGN.md §5n): split(PRNGKey(2^33 | seed), num_envs).  The root [2, seed]
-    differs from the trainer's [0, seed] and from the controllers' member keys [1, seed], so no chain shares a key with them."""
-    if not 0 <= int(seed) < 1 << 32:
-        raise ValueError(f"domain randomisation needs a seed in 0 .. 2^32 - 1 (got {seed})")
-    return prng.split(prng.PRNGKey((2 << 32) | int(seed)), num_envs)
-
-
-def check_randomization(randomization: Optional[dict], env) -> Optional[tuple]:
-    """the trainers' `randomization` argument checked on the host: None, or dict(friction_range=(lo, hi), gear_range=(lo, hi)) on an
-    xpbd env (either range may be omitted: (1, 1)).  Returns None or (friction_range, gear_range) as float32 pairs."""
-    if randomization is None:
-        return None
-    if not isinstance(randomization, dict) or set(randomization) - {"friction_range", "gear_range"}:
-        raise ValueError(f"randomization must be None or dict(friction_range=(lo, hi), gear_range=(lo, hi)) (got {randomization!r})")
-    if not isinstance(env, PipelineEnv):
-        raise ValueError(f"domain randomisation exists for the positional (xpbd) envs only, not {type(env).__name__}")
-    r = dr_range(randomization.get("friction_range", (1.0, 1.0)), randomization.get("gear_range", (1.0, 1.0)))
-    return (r[0], r[1]), (r[2], r[3])
 
 
 @dataclasses.dataclass
@@ -86,8 +64,7 @@ def key_chain(seed: int, c: Counts, num_envs: int, unroll_length: int, num_updat
     policy, value = split(global).  Per epoch `epoch_key, local = split(local)` and key = split(epoch_key, 1)[0]; per training step
     `key_sgd, key_unroll, key = split(key, 3)`; per unroll `cur, next = split(k)` and per unroll step `act, next = split(cur)`; per
     SGD epoch `key, key_perm, key_grad = split(key, 3)`, the permutation's rounds `k, sub = split(k)` and per minibatch
-    `k, key_loss = split(k)`.  The evaluator: per evaluation `eval_key, unroll_key = split(eval_key)`, reset keys split(unroll_key,
-    num_eval_envs) and act keys from unroll_key as an unroll."""
+    `k, key_loss = split(k)`.  The evaluator's keys are common.eval_keys of eval_key."""
     T, U, E = unroll_length, c.U, num_updates_per_batch
     gk, lk = prng.split(prng.PRNGKey(seed))
     lk = fold_in(lk, 0)
@@ -116,99 +93,45 @@ def key_chain(seed: int, c: Counts, num_envs: int, unroll_length: int, num_updat
                 for m in range(num_minibatches):
                     kgrad, loss[s, e * num_minibatches + m] = prng.split2(kgrad)
             s += 1
-    n_eval = c.num_evals_after_init + 1
-    eval_reset = np.zeros((n_eval, num_eval_envs, 2), np.uint32)
-    eval_act = np.zeros((n_eval, episode_length, 2), np.uint32)
-    for i in range(n_eval):
-        eval_key, uk = prng.split2(eval_key)
-        eval_reset[i] = prng.split(uk, num_eval_envs)
-        cur = uk
-        for t in range(episode_length):
-            eval_act[i, t], cur = prng.split2(cur)
+    eval_reset, eval_act = common.eval_keys(eval_key, c.num_evals_after_init + 1, num_eval_envs, episode_length)
     return Keys(kp, kv, prng.split(key_env, num_envs), act, perm, loss, eval_reset, eval_act)
 
 
-def _i32(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a, np.uint32).view(np.int32)).to(dev)
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else t.data_ptr()
-
-
 # ---- acting ------------------------------------------------------------------------------------------------------------------------
-class Actor:
-    """The stochastic policy on a VecEnv: `act(key)` writes tanh(raw) for every env into the VecEnv's actions (one mbd_ppo_act launch,
-    make_inference_fn(params)(obs, key) of Brax).  policy: flat fp32 cuda tensor; mean / std: [O] cuda tensors."""
+class Actor(common.Actor):
+    """PPO's stochastic policy on a VecEnv (common.Actor): one mbd_ppo_act launch per act()."""
+    EVAL, EVAL_RECORD = _lib.PPO_EVAL, _lib.PPO_EVAL_RECORD
 
-    def __init__(self, venv: VecEnv, policy: torch.Tensor, mean: torch.Tensor, std: torch.Tensor, keys: Optional[torch.Tensor] = None):
-        d = venv.device
-        self.own_key = keys is None       # no table: every act() is given its key
-        self.venv, self.keys = venv, (torch.zeros((1, 2), device=d, dtype=torch.int32) if keys is None else keys)
-        self.ctl = torch.zeros(4, device=d, dtype=torch.int32)
-        self.ret, self.active = torch.zeros(venv.num_envs, device=d), torch.ones(venv.num_envs, device=d)
-        self.policy, self.mean, self.std = policy, mean, std
-        P = _lib.PpoPlan()
-        P.B, P.O, P.nu, P.slots, P.act_key_rows = venv.num_envs, venv.spec.obs_size, venv.spec.nu, 1, self.keys.shape[0]
-        P.policy_dev, P.mean_dev, P.std_dev = policy.data_ptr(), mean.data_ptr(), std.data_ptr()
-        P.act_keys_dev, P.act_ctl_dev = self.keys.data_ptr(), self.ctl.data_ptr()
-        P.env_obs_dev, P.env_reward_dev, P.env_done_dev = venv.obs.data_ptr(), venv.reward.data_ptr(), venv.done.data_ptr()
-        P.env_trunc_dev, P.env_actions_dev = venv.truncation.data_ptr(), venv.actions.data_ptr()
-        P.ret_dev, P.active_dev = self.ret.data_ptr(), self.active.data_ptr()
-        self.plan = P
+    def _plan(self, B):
+        return _lib.PpoPlan(slots=1)
 
-    def start_eval(self):
-        """zero the episode returns, mark every env active and restart the key table"""
-        self.ret.zero_()
-        self.active.fill_(1.0)
-        self.ctl.zero_()
-
-    def act(self, key=None):
-        """one acting launch; `key` (uint32 [2]) replaces the table with that single key.  An actor built without a key table must be
-        given a key at every call (its one-row table is used up by the previous launch)."""
-        if key is None and self.own_key:
-            raise ValueError("this actor has no key table: pass the key of every act() call")
-        if key is not None:
-            self.keys[0].copy_(_i32(np.asarray(key).reshape(2), self.keys.device))
-            self.ctl.zero_()
-        with torch.cuda.device(self.venv.device):
-            ops.ppo_act(self.plan, _lib.PPO_EVAL)
-
-    def finish_eval(self) -> torch.Tensor:
-        """folds in the last step's reward; returns the episode returns [B]"""
-        with torch.cuda.device(self.venv.device):
-            ops.ppo_act(self.plan, _lib.PPO_EVAL_RECORD)
-        return self.ret
+    def _launch(self, mode):
+        ops.ppo_act(self.plan, mode)
 
 
 # ---- the trainer -------------------------------------------------------------------------------------------------------------------
-class PPOTrainer:
+class PPOTrainer(common.Trainer):
+    actor_cls = Actor
+
     def __init__(self, env, num_timesteps: int, episode_length: int, num_envs: int, num_eval_envs: int, learning_rate: float,
                  entropy_cost: float, discounting: float, seed: int, unroll_length: int, batch_size: int, num_minibatches: int,
                  num_updates_per_batch: int, num_evals: int, normalize_observations: bool, reward_scaling: float,
                  clipping_epsilon: float, gae_lambda: float, device=None, randomization: Optional[dict] = None):
-        self.dr = check_randomization(randomization, env)
-        _lib.require_gpu()
+        super().__init__(env, episode_length, num_envs, seed, device, randomization)
         if batch_size > _lib.PPO_MAX_MB:
             raise ValueError(f"batch_size (trajectories per minibatch) must be at most {_lib.PPO_MAX_MB}")
         self.c = c = counts(num_timesteps, num_envs, batch_size, num_minibatches, unroll_length, num_evals)
-        self.dev = d = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.env, self.B, self.T, self.U, self.mb, self.nmb, self.E = env, num_envs, unroll_length, c.U, batch_size, num_minibatches, num_updates_per_batch
-        self.episode_length, self.entropy_cost, self.clip = episode_length, entropy_cost, clipping_epsilon
+        self.T, self.U, self.mb, self.nmb, self.E = unroll_length, c.U, batch_size, num_minibatches, num_updates_per_batch
+        self.entropy_cost, self.clip = entropy_cost, clipping_epsilon
         self.normalize_observations = normalize_observations
         self.keys = key_chain(seed, c, num_envs, unroll_length, num_updates_per_batch, num_minibatches, num_eval_envs, episode_length)
-        self.dr_keys = dr_keys(seed, num_envs) if self.dr is not None else None
-        with torch.cuda.device(d):
+        with torch.cuda.device(self.dev):
             self._setup(num_eval_envs, learning_rate, discounting, reward_scaling, gae_lambda)
 
     def _setup(self, num_eval_envs, learning_rate, discounting, reward_scaling, gae_lambda):
         d, B, T, U, mb = self.dev, self.B, self.T, self.U, self.mb
-        self.venv = VecEnv(self.env, B, self.episode_length, device=d)
-        self.evenv = VecEnv(self.env, num_eval_envs, self.episode_length, device=d)
-        O, nu = self.venv.spec.obs_size, self.venv.spec.nu
-        if O > _lib.PPO_MAX_OBS or nu > _lib.PPO_MAX_NU:
-            raise ValueError(f"observation size {O} / action size {nu} above {_lib.PPO_MAX_OBS} / {_lib.PPO_MAX_NU}")
-        self.O, self.nu = O, nu
+        self._make_envs(num_eval_envs)
+        O, nu = self.O, self.nu
         self.psizes, self.vsizes = nets.policy_sizes(O, nu), nets.value_sizes(O)
         self.Np = nets.num_params(self.psizes)
         K = self.keys
@@ -239,30 +162,18 @@ class PPOTrainer:
                    "mbd_mnist_batch_indices")
         self.perm_scratch = torch.empty(int(nbytes.value), device=d, dtype=torch.uint8)
         self.perm_bytes = nbytes
-        v = self.venv
-        P = _lib.PpoPlan()
-        P.B, P.O, P.nu, P.slots, P.unroll, P.mb = B, O, nu, S, T, mb
+        P = common.acting_plan(_lib.PpoPlan(), self.venv, self.theta, self.mean, self.std, self.act_keys, self.act_ctl)
+        P.slots, P.unroll, P.mb = S, T, mb
         P.reward_scaling, P.discount, P.gae_lambda = reward_scaling, discounting, gae_lambda
-        P.act_key_rows, P.loss_key_rows = self.act_keys.shape[0], self.loss_keys.shape[0]
-        P.policy_dev, P.mean_dev, P.std_dev = self.theta.data_ptr(), self.mean.data_ptr(), self.std.data_ptr()
-        P.act_keys_dev, P.act_ctl_dev = self.act_keys.data_ptr(), self.act_ctl.data_ptr()
-        P.env_obs_dev, P.env_reward_dev, P.env_done_dev = v.obs.data_ptr(), v.reward.data_ptr(), v.done.data_ptr()
-        P.env_trunc_dev, P.env_actions_dev = v.truncation.data_ptr(), v.actions.data_ptr()
+        P.loss_key_rows = self.loss_keys.shape[0]
         P.obs_dev, P.raw_dev, P.logp_dev = self.obs.data_ptr(), self.raw.data_ptr(), self.logp.data_ptr()
         P.reward_dev, P.disc_dev, P.trunc_dev = self.reward.data_ptr(), self.disc.data_ptr(), self.trunc.data_ptr()
         P.stat_dev, P.stat_scratch_dev = self.stat.data_ptr(), self.stat_scratch.data_ptr()
         P.loss_keys_dev, P.loss_ctl_dev = self.loss_keys.data_ptr(), self.mb_ctl.data_ptr() + 4
         P.traj_dev, P.vs_dev, P.adv_dev, P.ent_eps_dev = self.sel.data_ptr(), self.vs.data_ptr(), self.adv.data_ptr(), self.ent_eps.data_ptr()
         self.plan = P
-        self.eval_keys = _i32(K.eval_act.reshape(-1, 2), d)
-        self.eval_reset = _i32(K.eval_reset, d)
-        self.actor = Actor(self.evenv, self.theta.detach()[:self.Np], self.mean, self.std, self.eval_keys)
-        if self.dr is not None:          # the training envs only: evaluation stays on the nominal model
-            self.venv.set_domain_randomization(*self.dr, self.dr_keys)
-        self.venv.reset(_i32(K.env, d))
-        self.step_index = 0
-        self.eval_index = 0
-        self._unroll_graph = self._sgd_graph = self._eval_graph = None
+        self._finish_setup(self.theta.detach()[:self.Np])
+        self._unroll_graph = self._sgd_graph = None
 
     # -- the pieces ------------------------------------------------------------------------------------------------------------------
     def unroll(self):
@@ -310,36 +221,13 @@ class PPOTrainer:
                                                       ctypes.c_void_p(self.perm_scratch.data_ptr()), ctypes.byref(self.perm_bytes),
                                                       ops._stream()), "mbd_mnist_batch_indices")
 
-    def capture(self):
-        """captures the unroll, the SGD minibatch step and the evaluation step as CUDA graphs.  The SGD step is warmed up on a side
-        stream first and every state it touched is restored, so capturing changes no result."""
-        with torch.cuda.device(self.dev):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.unroll()
-            self._unroll_graph = g
-            snap = [t.detach().clone() for t in (self.theta, self.mb_ctl, self.vs, self.adv, self.ent_eps, self.sel)]
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                for _ in range(2):
-                    self.sgd_step()
-            torch.cuda.current_stream().wait_stream(s)
-            with torch.no_grad():
-                for t, v in zip((self.theta, self.mb_ctl, self.vs, self.adv, self.ent_eps, self.sel), snap):
-                    t.copy_(v)
-                for st in self.opt.state[self.theta].values():
-                    st.zero_()
-                self.theta.grad.zero_()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.sgd_step()
-            self._sgd_graph = g
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.actor.act()
-                ops.vec_step(self.evenv.plan)
-            self._eval_graph = g
+    def _capture_training(self):
+        """captures the unroll and the SGD minibatch step as CUDA graphs.  The SGD step is warmed up on a side stream first and every
+        state it touched is restored, so capturing changes no result."""
+        self._unroll_graph = common.graph(self.unroll)
+        self._warm_up(self.sgd_step, (self.theta, self.mb_ctl, self.vs, self.adv, self.ent_eps, self.sel),
+                      lambda: [*self.opt.state[self.theta].values(), self.theta.grad])
+        self._sgd_graph = common.graph(self.sgd_step)
 
     def training_step(self):
         """Brax's training_step: U unrolls, the record of the last step, the statistics, E epochs of minibatch steps"""
@@ -356,24 +244,6 @@ class PPOTrainer:
             for _ in range(self.E * self.nmb):
                 self._sgd_graph.replay() if self._sgd_graph is not None else self.sgd_step()
         self.step_index += 1
-
-    def evaluate(self) -> float:
-        """Evaluator.run_evaluation: num_eval_envs envs from split(unroll_key, num_eval_envs), episode_length stochastic steps, the
-        mean return of every env's first episode (synchronises)"""
-        with torch.cuda.device(self.dev):
-            self.evenv.reset(self.eval_reset[self.eval_index])
-            self.actor.start_eval()
-            self.actor.ctl[1:2].fill_(self.eval_index * self.episode_length)
-            for _ in range(self.episode_length):
-                if self._eval_graph is not None:
-                    self._eval_graph.replay()
-                else:
-                    self.actor.act()
-                    ops.vec_step(self.evenv.plan)
-            ret = self.actor.finish_eval()
-            out = float(ret.mean().item())
-        self.eval_index += 1
-        return out
 
     def params(self) -> dict:
         th = self.theta.detach().cpu().numpy()
@@ -402,27 +272,4 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
     tr = PPOTrainer(env, num_timesteps, episode_length, num_envs, num_eval_envs, learning_rate, entropy_cost, discounting, seed,
                     unroll_length, batch_size, num_minibatches, num_updates_per_batch, num_evals, normalize_observations,
                     reward_scaling, clipping_epsilon, gae_lambda, randomization=randomization)
-    if capture:
-        tr.capture()
-    c = tr.c
-    metrics = {}
-    if num_evals > 1:
-        metrics = {"eval/episode_reward": tr.evaluate()}
-        progress_fn(0, metrics)
-    for _ in range(c.num_evals_after_init):
-        t0 = time.perf_counter()
-        for _ in range(c.steps_per_epoch):
-            tr.training_step()
-        torch.cuda.synchronize(tr.dev)
-        sps = c.steps_per_epoch * c.env_steps_per_training_step / (time.perf_counter() - t0)
-        metrics = {"eval/episode_reward": tr.evaluate(), "training/sps": sps}
-        progress_fn(tr.step_index * c.env_steps_per_training_step, metrics)
-    params = tr.params()
-
-    def make_inference_fn(p):
-        def make(venv: VecEnv) -> Actor:
-            d = venv.device
-            return Actor(venv, torch.from_numpy(p["policy"]).to(d), torch.from_numpy(p["mean"]).to(d), torch.from_numpy(p["std"]).to(d))
-        return make
-
-    return make_inference_fn, params, metrics
+    return common.run_training(tr, num_evals, progress_fn, capture)

@@ -16,7 +16,6 @@ update as target + tau (q - target) (torch's lerp; Brax writes target (1 - tau) 
 from __future__ import annotations
 
 import dataclasses
-import time
 from typing import Callable, Optional
 
 import numpy as np
@@ -25,10 +24,10 @@ import torch.nn.functional as F
 
 from .. import _lib, ops, prng
 from ..envs import get_env
-from ..envs.vec import VecEnv
 from ..prng import fold_in
+from . import common
 from . import networks as nets
-from .ppo import _i32, check_randomization, dr_keys
+from .common import _i32, dr_keys  # noqa: F401  (sac.dr_keys is public)
 
 ALPHA_LEARNING_RATE = 3e-4      # Brax's alpha optimiser is adam(3e-4) whatever learning_rate is
 
@@ -81,7 +80,7 @@ def key_chain(seed: int, c: Counts, num_envs: int, updates: int, num_eval_envs: 
     policy, q = split(global); the buffer key split(rb_key, 1)[0].  Prefill: `prefill_key, local = split(local)`, k = split(prefill_key,
     1)[0], per step `k, next = split(k)` and act with k.  Per epoch `epoch_key, local = split(local)`, k = split(epoch_key, 1)[0]; per
     training step `k, next = split(k)`, `experience_key, training_key = split(k)`; per update `key, key_alpha, key_critic, key_actor =
-    split(key, 4)` from training_key.  The evaluator is PPO's.  The training steps of all epochs and the update chains run as array
+    split(key, 4)` from training_key.  The evaluator's keys are common.eval_keys of eval_key.  The training steps of all epochs and the update chains run as array
     operations (split_many): a Python loop over the 3.3 M splits of the reference's hopper run takes about a minute."""
     gk, lk = prng.split(prng.PRNGKey(seed))
     lk = fold_in(lk, 0)
@@ -107,15 +106,7 @@ def key_chain(seed: int, c: Counts, num_envs: int, updates: int, num_eval_envs: 
     for g in range(updates):
         k4 = split_many(key, 4)
         key, noise[:, g] = k4[:, 0], k4[:, 1:]
-    n_eval = E + 1
-    eval_reset = np.zeros((n_eval, num_eval_envs, 2), np.uint32)
-    eval_act = np.zeros((n_eval, episode_length, 2), np.uint32)
-    for i in range(n_eval):
-        eval_key, uk = prng.split2(eval_key)
-        eval_reset[i] = prng.split(uk, num_eval_envs)
-        cur = uk
-        for t in range(episode_length):
-            eval_act[i, t], cur = prng.split2(cur)
+    eval_reset, eval_act = common.eval_keys(eval_key, E + 1, num_eval_envs, episode_length)
     return Keys(kp, kq, prng.split(env_key, num_envs), prng.split(rb_key, 1)[0], np.concatenate([pre, et[:, 0]]), noise,
                 eval_reset, eval_act)
 
@@ -257,79 +248,43 @@ LEARNERS = ("torch", "fused")
 
 
 # ---- acting ------------------------------------------------------------------------------------------------------------------------
-class Actor:
-    """The stochastic SAC policy on a VecEnv, with ppo.Actor's protocol: `act(key)` writes tanh(raw) for every env into the VecEnv's
-    actions (one mbd_sac_act launch, make_inference_fn(params)(obs, key) of Brax); start_eval / finish_eval accumulate the return of
-    every env's first episode.  policy: flat fp32 cuda tensor; mean / std: [O] cuda tensors."""
+class Actor(common.Actor):
+    """SAC's stochastic policy on a VecEnv (common.Actor): one mbd_sac_act launch per act()."""
+    EVAL, EVAL_RECORD = _lib.SAC_EVAL, _lib.SAC_EVAL_RECORD
 
-    def __init__(self, venv: VecEnv, policy: torch.Tensor, mean: torch.Tensor, std: torch.Tensor, keys: Optional[torch.Tensor] = None):
-        d = venv.device
-        self.own_key = keys is None
-        self.venv, self.keys = venv, (torch.zeros((1, 2), device=d, dtype=torch.int32) if keys is None else keys)
-        self.ctl = torch.zeros(4, device=d, dtype=torch.int32)
-        self.ret, self.active = torch.zeros(venv.num_envs, device=d), torch.ones(venv.num_envs, device=d)
-        self.policy, self.mean, self.std = policy, mean, std
-        P = _lib.SacPlan()
-        P.B, P.O, P.nu, P.capacity, P.act_key_rows = venv.num_envs, venv.spec.obs_size, venv.spec.nu, venv.num_envs, self.keys.shape[0]
-        P.policy_dev, P.mean_dev, P.std_dev = policy.data_ptr(), mean.data_ptr(), std.data_ptr()
-        P.act_keys_dev, P.act_ctl_dev = self.keys.data_ptr(), self.ctl.data_ptr()
-        P.env_obs_dev, P.env_reward_dev, P.env_done_dev = venv.obs.data_ptr(), venv.reward.data_ptr(), venv.done.data_ptr()
-        P.env_trunc_dev, P.env_actions_dev = venv.truncation.data_ptr(), venv.actions.data_ptr()
-        P.ret_dev, P.active_dev = self.ret.data_ptr(), self.active.data_ptr()
-        self.plan = P
+    def _plan(self, B):
+        return _lib.SacPlan(capacity=B)
 
-    def start_eval(self):
-        self.ret.zero_()
-        self.active.fill_(1.0)
-        self.ctl.zero_()
-
-    def act(self, key=None):
-        """one acting launch; `key` (uint32 [2]) replaces the table with that single key.  An actor built without a key table must be
-        given a key at every call."""
-        if key is None and self.own_key:
-            raise ValueError("this actor has no key table: pass the key of every act() call")
-        if key is not None:
-            self.keys[0].copy_(_i32(np.asarray(key).reshape(2), self.keys.device))
-            self.ctl.zero_()
-        with torch.cuda.device(self.venv.device):
-            ops.sac_act(self.plan, _lib.SAC_EVAL)
-
-    def finish_eval(self) -> torch.Tensor:
-        with torch.cuda.device(self.venv.device):
-            ops.sac_act(self.plan, _lib.SAC_EVAL_RECORD)
-        return self.ret
+    def _launch(self, mode):
+        ops.sac_act(self.plan, mode)
 
 
 # ---- the trainer -------------------------------------------------------------------------------------------------------------------
-class SACTrainer:
+class SACTrainer(common.Trainer):
+    actor_cls = Actor
+
     def __init__(self, env, num_timesteps: int, episode_length: int, num_envs: int, num_eval_envs: int, learning_rate: float,
                  discounting: float, seed: int, batch_size: int, num_evals: int, normalize_observations: bool, reward_scaling: float,
                  tau: float, min_replay_size: int, max_replay_size: int, grad_updates_per_step: int, device=None,
                  learner: str = "torch", randomization: Optional[dict] = None):
         if learner not in LEARNERS:
             raise ValueError(f"learner must be one of {LEARNERS}, not {learner!r}")
-        self.dr = check_randomization(randomization, env)
+        super().__init__(env, episode_length, num_envs, seed, device, randomization)
         self.learner_kind = learner
-        _lib.require_gpu()
         if not num_envs <= max_replay_size <= _lib.SAC_MAX_CAPACITY:
             raise ValueError(f"max_replay_size must be in num_envs..{_lib.SAC_MAX_CAPACITY}")
         self.c = c = counts(num_timesteps, num_envs, min_replay_size, num_evals)
-        self.dev = d = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.env, self.B, self.mb, self.G, self.cap = env, num_envs, batch_size, grad_updates_per_step, max_replay_size
-        self.episode_length, self.normalize_observations = episode_length, normalize_observations
+        self.mb, self.G, self.cap = batch_size, grad_updates_per_step, max_replay_size
+        self.normalize_observations = normalize_observations
         self.keys = key_chain(seed, c, num_envs, grad_updates_per_step, num_eval_envs, episode_length)
-        self.dr_keys = dr_keys(seed, num_envs) if self.dr is not None else None
-        with torch.cuda.device(d):
+        with torch.cuda.device(self.dev):
             self._setup(num_eval_envs, learning_rate, discounting, reward_scaling, tau)
 
     def _setup(self, num_eval_envs, learning_rate, discounting, reward_scaling, tau):
         d, B, G, mb, K = self.dev, self.B, self.G, self.mb, self.keys
-        self.venv = VecEnv(self.env, B, self.episode_length, device=d)
-        self.evenv = VecEnv(self.env, num_eval_envs, self.episode_length, device=d)
-        O, nu = self.venv.spec.obs_size, self.venv.spec.nu
-        if O > _lib.PPO_MAX_OBS or nu > _lib.PPO_MAX_NU:
-            raise ValueError(f"observation size {O} / action size {nu} above {_lib.PPO_MAX_OBS} / {_lib.PPO_MAX_NU}")
-        self.O, self.nu, self.R = O, nu, 2 * O + nu + 3
+        self._make_envs(num_eval_envs)
+        O, nu = self.O, self.nu
+        self.R = 2 * O + nu + 3
         psizes, qsizes = nets.sac_policy_sizes(O, nu), nets.sac_q_sizes(O, nu)
         if self.learner_kind == "fused":
             self.learner = FusedLearner(nets.init_params(K.policy, psizes), nets.sac_q_init(K.q, qsizes), O, nu, learning_rate,
@@ -355,14 +310,8 @@ class SACTrainer:
         self.upd_ctl = torch.zeros(1, device=d, dtype=torch.int64)
         if self.learner_kind == "fused":
             self.learner.bind(self.batch, self.eps, self.upd_ctl, self.mean, self.std)
-        v = self.venv
-        P = _lib.SacPlan()
-        P.B, P.O, P.nu, P.capacity, P.batch, P.updates = B, O, nu, self.cap, mb, G
-        P.act_key_rows, P.noise_key_rows = self.act_keys.shape[0], K.noise.shape[0]
-        P.policy_dev, P.mean_dev, P.std_dev = self.learner.policy.data_ptr(), self.mean.data_ptr(), self.std.data_ptr()
-        P.act_keys_dev, P.act_ctl_dev = self.act_keys.data_ptr(), self.act_ctl.data_ptr()
-        P.env_obs_dev, P.env_reward_dev, P.env_done_dev = v.obs.data_ptr(), v.reward.data_ptr(), v.done.data_ptr()
-        P.env_trunc_dev, P.env_actions_dev = v.truncation.data_ptr(), v.actions.data_ptr()
+        P = common.acting_plan(_lib.SacPlan(), self.venv, self.learner.policy, self.mean, self.std, self.act_keys, self.act_ctl)
+        P.capacity, P.batch, P.updates, P.noise_key_rows = self.cap, mb, G, K.noise.shape[0]
         P.stage_obs_dev, P.ring_dev, P.ring_ctl_dev, P.sample_ctl_dev = (t.data_ptr() for t in (self.stage, self.ring, self.ring_ctl,
                                                                                                   self.sample_ctl))
         P.noise_keys_dev, P.idx_dev, P.batch_dev, P.eps_dev = (t.data_ptr() for t in (self.noise_keys, self.idx, self.batch, self.eps))
@@ -372,15 +321,8 @@ class SACTrainer:
         S.obs_dev, S.stat_dev, S.stat_scratch_dev = self.stage.data_ptr(), self.stat.data_ptr(), self.stat_scratch.data_ptr()
         S.mean_dev, S.std_dev = self.mean.data_ptr(), self.std.data_ptr()
         self.stat_plan = S
-        self.eval_keys = _i32(K.eval_act.reshape(-1, 2), d)
-        self.eval_reset = _i32(K.eval_reset, d)
-        self.actor = Actor(self.evenv, self.learner.policy.detach(), self.mean, self.std, self.eval_keys)
-        if self.dr is not None:          # the training envs only: evaluation stays on the nominal model
-            self.venv.set_domain_randomization(*self.dr, self.dr_keys)
-        self.venv.reset(_i32(K.env, d))
-        self.step_index = 0
-        self.eval_index = 0
-        self._act_graph = self._sample_graph = self._sgd_graph = self._eval_graph = None
+        self._finish_setup(self.learner.policy.detach())
+        self._act_graph = self._sample_graph = self._sgd_graph = None
 
     # -- the pieces ------------------------------------------------------------------------------------------------------------------
     def actor_step(self):
@@ -413,49 +355,17 @@ class SACTrainer:
             for _ in range(self.c.prefill_steps):
                 self._act_graph.replay() if self._act_graph is not None else self.actor_step()
 
-    def capture(self):
-        """captures the acting step, the sampling and one update as CUDA graphs (and the evaluation step).  The torch update is
-        warmed up on a side stream first and every state it touched is restored, so capturing changes no result; the fused update is
-        two kernel launches and is captured without running."""
-        with torch.cuda.device(self.dev):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.actor_step()
-            self._act_graph = g
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.sample()
-            self._sample_graph = g
-            if self.learner_kind == "torch":
-                self._warm_torch_update()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.sgd_step()
-            self._sgd_graph = g
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.actor.act()
-                ops.vec_step(self.evenv.plan)
-            self._eval_graph = g
-
-    def _warm_torch_update(self):
-        """two torch updates on a side stream (the optimisers allocate their state), then every state they touched restored"""
-        L = self.learner
-        kept = (L.policy, L.q, L.target_q, L.log_alpha, self.upd_ctl)
-        snap = [t.detach().clone() for t in kept]
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                self.sgd_step()
-        torch.cuda.current_stream().wait_stream(s)
-        with torch.no_grad():
-            for t, v in zip(kept, snap):
-                t.copy_(v)
-            for t in L.state()[4:]:     # the optimisers' moments and step counts
-                t.zero_()
-            for t in (L.policy.grad, L.q.grad, L.log_alpha.grad):
-                t.zero_()
+    def _capture_training(self):
+        """captures the acting step, the sampling and one update as CUDA graphs.  The torch update is warmed up on a side stream
+        first and every state it touched is restored, so capturing changes no result; the fused update is two kernel launches and is
+        captured without running."""
+        self._act_graph = common.graph(self.actor_step)
+        self._sample_graph = common.graph(self.sample)
+        if self.learner_kind == "torch":
+            L = self.learner              # L.state()[4:]: the optimisers' moments and step counts
+            self._warm_up(self.sgd_step, (L.policy, L.q, L.target_q, L.log_alpha, self.upd_ctl),
+                          lambda: [*L.state()[4:], L.policy.grad, L.q.grad, L.log_alpha.grad])
+        self._sgd_graph = common.graph(self.sgd_step)
 
     def training_step(self):
         """Brax's training_step: an actor step, the replay sample, grad_updates_per_step updates"""
@@ -469,25 +379,8 @@ class SACTrainer:
         self.step_index += 1
 
     def env_steps(self) -> int:
+        """Brax's count includes the prefill"""
         return self.c.prefill_env_steps + self.step_index * self.B
-
-    def evaluate(self) -> float:
-        """Evaluator.run_evaluation (PPO's): num_eval_envs envs, episode_length stochastic steps, the mean return of every env's
-        first episode (synchronises)"""
-        with torch.cuda.device(self.dev):
-            self.evenv.reset(self.eval_reset[self.eval_index])
-            self.actor.start_eval()
-            self.actor.ctl[1:2].fill_(self.eval_index * self.episode_length)
-            for _ in range(self.episode_length):
-                if self._eval_graph is not None:
-                    self._eval_graph.replay()
-                else:
-                    self.actor.act()
-                    ops.vec_step(self.evenv.plan)
-            ret = self.actor.finish_eval()
-            out = float(ret.mean().item())
-        self.eval_index += 1
-        return out
 
     def params(self) -> dict:
         L = self.learner
@@ -519,28 +412,4 @@ def train(environment, num_timesteps: int, episode_length: int, action_repeat: i
     tr = SACTrainer(env, num_timesteps, episode_length, num_envs, num_eval_envs, learning_rate, discounting, seed, batch_size, num_evals,
                     normalize_observations, reward_scaling, tau, min_replay_size, max_replay_size, grad_updates_per_step,
                     learner=learner, randomization=randomization)
-    if capture:
-        tr.capture()
-    c = tr.c
-    metrics = {}
-    if num_evals > 1:
-        metrics = {"eval/episode_reward": tr.evaluate()}
-        progress_fn(0, metrics)
-    tr.prefill()
-    for _ in range(c.num_evals_after_init):
-        t0 = time.perf_counter()
-        for _ in range(c.steps_per_epoch):
-            tr.training_step()
-        torch.cuda.synchronize(tr.dev)
-        sps = c.steps_per_epoch * c.env_steps_per_training_step / (time.perf_counter() - t0)
-        metrics = {"eval/episode_reward": tr.evaluate(), "training/sps": sps}
-        progress_fn(tr.env_steps(), metrics)
-    params = tr.params()
-
-    def make_inference_fn(p):
-        def make(venv: VecEnv) -> Actor:
-            d = venv.device
-            return Actor(venv, torch.from_numpy(p["policy"]).to(d), torch.from_numpy(p["mean"]).to(d), torch.from_numpy(p["std"]).to(d))
-        return make
-
-    return make_inference_fn, params, metrics
+    return common.run_training(tr, num_evals, progress_fn, capture)

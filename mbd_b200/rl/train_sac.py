@@ -42,7 +42,7 @@ def main(argv=None):
 
     from ..envs import get_env
     from . import sac
-    from .ppo import check_randomization
+    from .common import check_randomization
     from .train_brax import post_training, progress_printer, randomization
 
     env = get_env(a.env_name)
