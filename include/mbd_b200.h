@@ -120,7 +120,8 @@ int mbd_weighted_sqerr_sum(const float* weights_dev, const float* Y0s_dev, const
  * div_nn_ (18), sqrt_ (19) and the low / high halves of their two-lane forms, paired like ops 5 and 6: rcp_ (20 / 21),
  * div_ (22 / 23), div_nn_ (24 / 25), sqrt_ (26 / 27);  and planted mistakes that exist only here, each a spec function
  * with one step removed: the sine without its third Cody-Waite constant (28), mbd_expf without its second (29), rcp as the
- * bare rcp.approx seed (30), sqrt without its final FMA (31), a division returning a * r after one Newton step (32). */
+ * bare rcp.approx seed (30), sqrt without its final FMA (31), a division returning a * r after one Newton step (32), sqrt
+ * without the exact scaling of arguments below 2^-100 (33). */
 int mbd_test_arith(int op, const float* a_dev, const float* b_dev, float* out_dev, int n, mbd_stream s);
 
 /* Test hook: err_dev[i] (double) = the error of op (as mbd_test_arith) at (a[i], b[i]) against a float64 reference from

@@ -152,18 +152,13 @@ MBD_HD void mbd_sac_adam_scalars(float lr, long long t, float* step, float* bc2s
   *step = MBD_DIV(lr, bc1);
   *bc2s = MBD_SQRT(bc2);
 }
-/* sqrt of Adam's second moment.  MBD_SQRT's device sequence is not defined below FLT_MIN: rsqrt.approx.ftz flushes a subnormal
- * to 0, and the Newton step then computes inf * 0 = NaN.  v reaches the subnormal range when a parameter's gradient stays tiny or
- * rarely non-zero (v decays by 0.999 each update), so a subnormal v is scaled by 2^24 first and its root by 2^-12.  Both
- * scalings are exact, so the result is still the correctly rounded sqrt(v) on both sides. */
-MBD_HD float mbd_sac_sqrt_v(float v) {
-  return v < 1.17549435e-38f ? MBD_SQRT(v * 16777216.0f) * 2.44140625e-4f : MBD_SQRT(v);
-}
-/* m = m + (1 - b1) (g - m) (torch's lerp_); v = v b2 + (1 - b2) g^2; p = p - step * (m / (sqrt(v) / bc2s + eps)) */
+/* m = m + (1 - b1) (g - m) (torch's lerp_); v = v b2 + (1 - b2) g^2; p = p - step * (m / (sqrt(v) / bc2s + eps)).  v reaches the
+ * subnormal range when a parameter's gradient stays tiny or rarely non-zero (v decays by 0.999 each update); MBD_SQRT is
+ * correctly rounded there too (include/mbd_fp32.h). */
 MBD_HD void mbd_sac_adam(float* p, float* m, float* v, float g, float step, float bc2s) {
   const float mm = *m + 0.1f * (g - *m);
   const float vv = *v * 0.999f + 0.001f * (g * g);
-  const float denom = MBD_DIV(mbd_sac_sqrt_v(vv), bc2s) + MBD_SAC_ADAM_EPS;
+  const float denom = MBD_DIV(MBD_SQRT(vv), bc2s) + MBD_SAC_ADAM_EPS;
   *m = mm;
   *v = vv;
   *p = *p - step * MBD_DIV(mm, denom);

@@ -37,9 +37,9 @@ template <class T> PK_FN T vdot(V<T> a, V<T> b) { return fma(a.z, b.z, fma(a.y, 
 template <class T> PK_FN V<T> vcross(V<T> a, V<T> b) {
   return mkV(fma(a.y, b.z, neg(mul(a.z, b.y))), fma(a.z, b.x, neg(mul(a.x, b.z))), fma(a.x, b.y, neg(mul(a.y, b.x))));
 }
-template <class T> PK_FN V<T> vnormalize(V<T> a, T* norm) {
+template <class T, bool kExact = false> PK_FN V<T> vnormalize(V<T> a, T* norm) {   // kExact: sqrt_x (pk_scalar.cuh)
   const T zero = bc<T>(0.0f);
-  T n = sqrt_(vdot(a, a));
+  T n = kExact ? sqrt_x(vdot(a, a)) : sqrt_(vdot(a, a));
   T inv = sel(eq(n, zero), zero, rcp_(n));
   *norm = n;
   return vscale(a, inv);
@@ -193,7 +193,7 @@ PK_FN void contact_position_plane(const Model<T>& M, int l, int ci, T im, V<T> p
   V<T> rl = vinv_rotate(r, q);
   V<T> pbar = vadd(p_prev, vrotate(rl, q_prev));
   T dx = sub(cp.x, pbar.x), dy = sub(cp.y, pbar.y);
-  T ct = sqrt_(fma(dy, dy, mul(dx, dx)));
+  T ct = sqrt_x(fma(dy, dy, mul(dx, dx)));
   T inv = sel(eq(ct, zero), zero, rcp_(ct));
   T ntx = mul(dx, inv), nty = mul(dy, inv);
   T c1 = neg(mul(r.z, nty)), c2 = mul(r.z, ntx), c3 = fma(r.x, nty, neg(mul(r.y, ntx)));
@@ -217,7 +217,7 @@ PK_FN void contact_velocity_plane(const Model<T>& M, int l, int ci, T im, T inv_
   V<T> r = vsub(cp, p);
   V<T> rel = vadd(v, vcross(w, r));   // v is a product (project_xd)
   T vn = rel.z;
-  T vtn = sqrt_(fma(rel.y, rel.y, mul(rel.x, rel.x)));
+  T vtn = sqrt_x(fma(rel.y, rel.y, mul(rel.x, rel.x)));
   T inv = sel(eq(vtn, zero), zero, rcp_(vtn));
   T tdx = mul(rel.x, inv), tdy = mul(rel.y, inv);
   T fr = mul(mul(mu, abs_(dl)), inv_dt);
@@ -315,7 +315,7 @@ PK_FN void phase_C(const Model<T>& M, const Cfg& c, const Smem<T>& S, State<T>& 
     V<T> rcw = vrotate(M.l3(MBD_F_RC, c.l), s.q);
     V<T> e = vsub(vadd(s.p, rcw), vadd(pp, rpw));
     T cn;
-    V<T> n = vnormalize(e, &cn);
+    V<T> n = vnormalize<T, true>(e, &cn);
     V<T> crc = vcross(rcw, n), crp = vcross(rpw, n);
     T w_c = add(im_c, vdot(crc, crc));
     T w_p = fma(ii_p, vdot(crp, crp), im_p);

@@ -6,7 +6,8 @@ constants to these functions; the kernels run the nvcc build.  A unary fp32 func
 evaluates all of those in each charged range beside a float64 reference from CUDA's double libm (mbd_test_sweep) and the
 constants become proofs for the build that runs.  atan2 takes two operands: its polynomial and quadrant roundings are swept
 exhaustively with a divisor of 1 (the quotient is exact) and the rounding of a general quotient is added analytically.  The
-exact division, reciprocal and square root are held bit for bit to the correctly rounded result on their documented domain.
+exact division, reciprocal and square root are held bit for bit to the correctly rounded result on their documented domain,
+which includes every subnormal and tiny operand the host accepts.
 Run with -s to see the measured maxima, their input bits, the planted-mistake margins and the table of what the exact
 operations do outside their domain.
 """
@@ -34,13 +35,15 @@ FLT_MAX = float(np.finfo(f32).max)
 OP = dict(div=0, rcp=1, sqrt=2, atan2=3, pk_atan2=4, pk_atan2_lo=5, pk_atan2_hi=6, log=7, exp=8, sin=9, cos=10, erfinv=11,
           normal=12, tanh=13, softplus=14, swish=15, pk_rcp=16, pk_div=17, pk_div_nn=18, pk_sqrt=19, pk_rcp_lo=20, pk_rcp_hi=21,
           pk_div_lo=22, pk_div_hi=23, pk_div_nn_lo=24, pk_div_nn_hi=25, pk_sqrt_lo=26, pk_sqrt_hi=27,
-          planted_sin=28, planted_exp=29, planted_rcp=30, planted_sqrt=31, planted_div=32)
+          planted_sin=28, planted_exp=29, planted_rcp=30, planted_sqrt=31, planted_div=32, planted_sqrt_noscale=33)
 # the metrics of mbd_test_err: ulps of fl(ref), u |ref|, u (1 + |ref|), u, u |x|, exact, atan2 composed with its quotient
 ULP, REL, ONEPLUS, ABS, XREL, EXACT, ATANC = range(7)
 RCP_OPS = ("rcp", "pk_rcp", "pk_rcp_lo", "pk_rcp_hi")
 SQRT_OPS = ("sqrt", "pk_sqrt", "pk_sqrt_lo", "pk_sqrt_hi")
 DIV_OPS = ("div", "pk_div", "pk_div_lo", "pk_div_hi")             # any divisor sign
 DIV_NN_OPS = ("pk_div_nn", "pk_div_nn_lo", "pk_div_nn_hi")        # divisor >= +0 (atan2_'s |.| / |.|)
+# the packed kernel's two-lane rcp_ / div_ / div_nn_ / sqrt_ keep the bare fast path (csrc/pk_scalar.cuh): exact on its domain only
+FAST_ONLY = ("pk_rcp_lo", "pk_rcp_hi", "pk_sqrt_lo", "pk_sqrt_hi", "pk_div_lo", "pk_div_hi", "pk_div_nn_lo", "pk_div_nn_hi")
 
 # name: (op, metric, intervals, bound in the metric's unit).  Every float32 of every interval is evaluated.
 UNARY = {
@@ -250,28 +253,33 @@ def _exact(results, what):
 
 
 def test_rcp_exact():
-    """every float32 with |x| in [2^-101, 2^126], both signs: the device reciprocal, the packed kernel's scalar rcp_ and both
-    halves of its two-lane form are the correctly rounded 1 / x"""
+    """every nonzero float32 with |x| <= 2^126, both signs, subnormals included: the device reciprocal and the packed kernel's
+    scalar rcp_ are the correctly rounded 1 / x, which is +-inf below the overflow edge near 2^-128; both halves of rcp_'s
+    two-lane form are, for every |x| in [2^-101, 2^126]"""
     jobs, names = [], []
+    tiny = float(x32(1))
     for op in RCP_OPS:
-        for first, count in span(2.0 ** -101, 2.0 ** 126) + span(-(2.0 ** 126), -(2.0 ** -101)):
+        lo = 2.0 ** -101 if op in FAST_ONLY else tiny
+        for first, count in span(lo, 2.0 ** 126) + span(-(2.0 ** 126), -lo):
             jobs.append((op, EXACT, first, count, 0.0, False))
             names.append(f"{op} from 0x{first:08x}")
     res = sweep(jobs)
-    assert sum(r[3] for r in res) == 8 * (b32(2.0 ** 126) - b32(2.0 ** -101) + 1)
+    assert sum(r[3] for r in res) == 4 * b32(2.0 ** 126) + 4 * (b32(2.0 ** 126) - b32(2.0 ** -101) + 1)
     _exact(zip(names, res), "rcp")
 
 
 def test_sqrt_exact():
-    """every float32 in the documented domain [2^-101, 2^126], and 0: the device square root, the packed kernel's scalar sqrt_ and
-    both halves of its two-lane form are the correctly rounded sqrt.  (Near 2^-126 the residual x - s^2 of the last Newton step
-    falls below the normal range and some results are 1 ulp off: test_exact_ops_outside_their_domain.)"""
+    """every float32 in [0, FLT_MAX], subnormals included: the device square root and the packed kernel's scalar sqrt_ are the
+    correctly rounded sqrt (arguments below 2^-100 through the exact scaling by 2^126); both halves of sqrt_'s two-lane form
+    are, for 0 and every x in [2^-101, FLT_MAX]"""
     jobs, names = [], []
     for op in SQRT_OPS:
-        for first, count in [(0, 1)] + span(2.0 ** -101, 2.0 ** 126):
+        for first, count in [(0, 1)] + span(2.0 ** -101 if op in FAST_ONLY else float(x32(1)), FLT_MAX):
             jobs.append((op, EXACT, first, count, 0.0, False))
             names.append(f"{op} from 0x{first:08x}")
-    _exact(zip(names, sweep(jobs)), "sqrt")
+    res = sweep(jobs)
+    assert sum(r[3] for r in res) == 2 * 0x7f800000 + 2 * (0x7f800000 - b32(2.0 ** -101) + 1)
+    _exact(zip(names, res), "sqrt")
 
 
 def _dividends(rng, n, emin, emax):
@@ -325,9 +333,8 @@ def _midpoint_pairs(rng, n):
 def test_div_exact():
     """the device division, the packed kernel's scalar div_ and div_nn_ and both halves of their two-lane forms are the correctly
     rounded quotient: every divisor mantissa against 1024 dividends, zero dividends of both signs, quotients constructed next to
-    rounding midpoints, and the edges of the domain (divisor in [2^-101, 2^126], dividend 0 or at least 2^-101 in magnitude,
-    quotient normal).  Below 2^-101 the remainder a - b q of the correction step loses bits to underflow
-    (test_exact_ops_outside_their_domain)."""
+    rounding midpoints, and the edges of the domain (0 < |divisor| <= 2^126, the quotient 0 or normal): divisors and dividends
+    below 2^-100, which take the exact scaling by 2^64, down to every subnormal (test_div_tiny_operands)."""
     rng = np.random.default_rng(12)
     res = sweep(_div_jobs(np.concatenate([_dividends(rng, 1024, -20, 20), f32([0.0, -0.0])]), 0))
     assert len(res) == 1026 * 11
@@ -351,32 +358,74 @@ def test_div_exact():
     print(f"\ndivision: {1026 * 11 + 5 * 16 * 11} divisor-mantissa sweeps and {a.size} near-midpoint quotients per op correctly rounded")
 
 
-def test_exact_ops_outside_their_domain():
-    """What the exact operations do outside the documented domain (subnormal operands and results under the .ftz seeds, divisors
-    above 2^126, dividends and square-root arguments whose Newton residual underflows): recorded, not asserted"""
-    rows = [
-        ("rcp, |x| subnormal", "rcp", 1, 0x007fffff, 0.0, False),
-        ("rcp, |x| in [2^-126, 2^-101)", "rcp", 0x00800000, b32(2.0 ** -101) - 0x00800000, 0.0, False),
-        ("rcp, |x| in (2^126, FLT_MAX]", "rcp", b32(2.0 ** 126) + 1, 0x7f7fffff - b32(2.0 ** 126), 0.0, False),
-        ("sqrt, x subnormal", "sqrt", 1, 0x007fffff, 0.0, False),
-        ("sqrt, x in [2^-126, 2^-125)", "sqrt", 0x00800000, 1 << 23, 0.0, False),
-        ("sqrt, x in [2^-125, 2^-113)", "sqrt", 0x01000000, 12 << 23, 0.0, False),
-        ("sqrt, x in [2^-113, 2^-101)", "sqrt", 0x07000000, 12 << 23, 0.0, False),
-        ("sqrt, x in (2^126, FLT_MAX]", "sqrt", b32(2.0 ** 126) + 1, 0x7f7fffff - b32(2.0 ** 126), 0.0, False),
-        ("div 1 / b, b in (2^126, FLT_MAX]", "div", b32(2.0 ** 126) + 1, 0x7f7fffff - b32(2.0 ** 126), 1.0, True),
-        ("div 1e-30 / b, b subnormal", "div", 1, 0x007fffff, 1e-30, True),
-        ("div 2^-120 / b, b in [2^10, 2^11): quotient subnormal", "div", b32(1024.0), 1 << 23, 2.0 ** -120, True),
-        ("div 1.3 2^-125 / b, b in [1, 2)", "div", b32(1.0), 1 << 23, float(f32(1.3) * f32(2.0 ** -125)), True),
-        ("div 1.3 2^-110 / b, b in [1, 2)", "div", b32(1.0), 1 << 23, float(f32(1.3) * f32(2.0 ** -110)), True),
-        ("div 1.3 2^-104 / b, b in [1, 2)", "div", b32(1.0), 1 << 23, float(f32(1.3) * f32(2.0 ** -104)), True),
-        ("div 1.3 2^-103 / b, b in [1, 2)", "div", b32(1.0), 1 << 23, float(f32(1.3) * f32(2.0 ** -103)), True),
-        ("div 1.3 2^-102 / b, b in [1, 2)", "div", b32(1.0), 1 << 23, float(f32(1.3) * f32(2.0 ** -102)), True),
-        ("div 3 2^-131 / b, b in [2^-20, 2^-19): dividend subnormal", "div", b32(2.0 ** -20), 1 << 23, 3 * 2.0 ** -131, True),
+def _div_tiny_jobs():
+    """(name, job) of every op of the division on sweeps with an operand below 2^-100: (sweep, first bits, count, other operand,
+    other first), expanded over the ops (div_nn_ only where the divisor is positive)"""
+    t = lambda e, m=1.0: float(f32(m) * f32(2.0 ** e))   # noqa: E731
+    specs = [
+        ("every subnormal divisor, dividend 1e-30", 1, 0x7fffff, 1e-30, True),
+        ("every subnormal divisor, dividend 1.3 2^-140", 1, 0x7fffff, t(-140, 1.3), True),
+        ("every subnormal divisor, dividend 0.75 (overflow below ~2^-127)", 1, 0x7fffff, 0.75, True),
+        ("divisors in [2^-126, 2^-101), dividend -1.7 2^-110", 0x00800000, b32(2.0 ** -101) - 0x00800000, t(-110, -1.7), True),
+        ("divisors in [2^-126, 2^-101), dividend 2^-3", 0x00800000, b32(2.0 ** -101) - 0x00800000, 0.125, True),
+        ("every subnormal dividend, divisor 2^-30", 1, 0x7fffff, t(-30), False),
+        ("every subnormal dividend, divisor -1.3 2^-27", 1, 0x7fffff, t(-27, -1.3), False),
+        ("every subnormal dividend, divisor 2^-140", 1, 0x7fffff, t(-140), False),
+        ("every subnormal dividend, divisor 1.1 2^-110", 1, 0x7fffff, t(-110, 1.1), False),
+        ("dividends in [2^-126, 2^-101), divisor 1", 0x00800000, b32(2.0 ** -101) - 0x00800000, 1.0, False),
+        ("dividends in [2^-126, 2^-101), divisor -0.7", 0x00800000, b32(2.0 ** -101) - 0x00800000, -0.7, False),
+        ("dividends in [2^-126, 2^-101), divisor 1.5 2^-120", 0x00800000, b32(2.0 ** -101) - 0x00800000, t(-120, 1.5), False),
+        ("divisors in [1, 2), dividend 1.3 2^-125", b32(1.0), 1 << 23, t(-125, 1.3), True),
+        ("divisors in [1, 2), dividend 1.3 2^-102", b32(1.0), 1 << 23, t(-102, 1.3), True),
+        ("divisors in [2^-20, 2^-19), dividend 3 2^-131", b32(2.0 ** -20), 1 << 23, 3 * 2.0 ** -131, True),
     ]
+    out = []
+    for name, first, count, other, of in specs:
+        for sign in (0, 0x80000000) if of else (0,):
+            for op in tuple(o for o in DIV_OPS + (DIV_NN_OPS if (sign == 0 if of else other > 0) else ()) if o not in FAST_ONLY):
+                out.append((f"{op}: {name}{', negative divisor' if sign else ''}", (op, EXACT, first | sign, count, other, of)))
+    return out
+
+
+def test_div_tiny_operands():
+    """divisors and dividends below 2^-101, subnormals included, wherever the quotient is normal (or overflows for a subnormal
+    divisor): the device division and the packed kernel's scalar div_ and div_nn_ are correctly rounded through the exact
+    scaling by 2^64"""
+    jobs = _div_tiny_jobs()
+    res = sweep([j for _, j in jobs])
+    _exact(zip([n for n, _ in jobs], res), "div")
+    print(f"\ndivision with tiny operands: {sum(r[3] for r in res)} quotients correctly rounded")
+
+
+def test_exact_ops_outside_their_domain():
+    """What the exact operations do outside the documented domain (reciprocals and quotients in the subnormal range under the
+    .ftz seed, divisors above 2^126), and the packed kernel's two-lane rcp_ / div_ / sqrt_ / atan2_ below 2^-101: recorded, not
+    asserted"""
+    rows = [
+        ("rcp, |x| in (2^126, FLT_MAX]: 1 / x subnormal", "rcp", b32(2.0 ** 126) + 1, 0x7f7fffff - b32(2.0 ** 126), 0.0, False),
+        ("div 1 / b, b in (2^126, FLT_MAX]", "div", b32(2.0 ** 126) + 1, 0x7f7fffff - b32(2.0 ** 126), 1.0, True),
+        ("div 2^-120 / b, b in [2^10, 2^11): quotient subnormal", "div", b32(1024.0), 1 << 23, 2.0 ** -120, True),
+        ("div a / 2^20, a subnormal: quotient subnormal", "div", 1, 0x7fffff, 2.0 ** 20, False),
+    ] + [(f"{op}, x subnormal (bare fast path)", op, 1, 0x7fffff, 0.0, False) for op in FAST_ONLY if "div" not in op] + [
+        (f"{op}, x in [2^-126, 2^-101) (bare fast path)", op, 0x00800000, b32(2.0 ** -101) - 0x00800000, 0.0, False)
+        for op in FAST_ONLY if "div" not in op] + [
+        (f"{op} 1e-30 / b, b subnormal (bare fast path)", op, 1, 0x7fffff, 1e-30, True) for op in FAST_ONLY if "div" in op] + [
+        (f"{op} 1.3 2^-110 / b, b in [1, 2) (bare fast path)", op, b32(1.0), 1 << 23, float(f32(1.3) * f32(2.0 ** -110)), True)
+        for op in FAST_ONLY if "div" in op]
     res = sweep([(op, EXACT, first, count, other, of) for _, op, first, count, other, of in rows])
+    # the two-lane atan2_ divides with the bare div_nn_: against mbd_atan2f on (y, x) with both magnitudes in one band
+    rng = np.random.default_rng(16)
+    lanes = []
+    for band, (lo, hi) in (("subnormal", (1, 0x7fffff)), ("[2^-126, 2^-101)", (0x00800000, b32(2.0 ** -101) - 1))):
+        y, x = (rng.integers(lo, hi + 1, 1 << 16).astype(np.uint32).view(f32) * rng.choice(f32([-1, 1]), 1 << 16) for _ in range(2))
+        ref = arith("atan2", y, x)
+        for op in ("pk_atan2_lo", "pk_atan2_hi"):
+            got = arith(op, y, x)
+            lanes.append(f"{op}, |y| and |x| {band:17s} {np.count_nonzero(~np.isfinite(got)):>6d} of {y.size} not finite, "
+                         f"{np.count_nonzero(got.view(np.uint32) != ref.view(np.uint32)):>6d} differ from mbd_atan2f")
     _show("exact operations outside their domain (not asserted)",
           [f"{name:56s} {cnt:>10d} of {n:>10d} not correctly rounded, worst {e:.4g} ulp at 0x{bits:08x}"
-           for (name, *_), (e, bits, cnt, n) in zip(rows, res)])
+           for (name, *_), (e, bits, cnt, n) in zip(rows, res)] + lanes)
     assert all(r[3] > 0 for r in res)
 
 
@@ -473,17 +522,19 @@ def test_reference_agrees_with_numpy(unary):
 
 
 def test_planted_mistakes_fail():
-    """each planted mistake (a spec function with one step removed, include/mbd_b200.h ops 28-32) fails the check its function
+    """each planted mistake (a spec function with one step removed, include/mbd_b200.h ops 28-33) fails the check its function
     passes"""
     sin = sweep_unary("planted_sin", ABS, UNARY["sin"][2])
     exp = sweep_unary("planted_exp", REL, UNARY["exp"][2])
-    ex = sweep([("planted_rcp", EXACT, b32(1.0), 1 << 23, 0.0, False), ("planted_sqrt", EXACT, b32(1.0), 1 << 24, 0.0, False)]
+    ex = sweep([("planted_rcp", EXACT, b32(1.0), 1 << 23, 0.0, False), ("planted_sqrt", EXACT, b32(1.0), 1 << 24, 0.0, False),
+                ("planted_sqrt_noscale", EXACT, 1, 0x7fffff, 0.0, False)]
                + [("planted_div", EXACT, b32(1.0), 1 << 23, float(a), True) for a in _dividends(np.random.default_rng(15), 16, -20, 20)])
-    div = worst(ex[2:])
+    div = worst(ex[3:])
     rows = [f"sin without its 3rd Cody-Waite constant: {sin[0] * U:.4g} absolute at 0x{sin[1]:08x}, {sin[0] * U / COS_ABS_ERR:.4g} x COS_ABS_ERR",
             f"exp without its 2nd Cody-Waite constant: {exp[0]:.4g} u|ref| at 0x{exp[1]:08x}, {exp[0] / rl_ref.EXP_REL:.4g} x EXP_REL"]
-    for what, r in (("rcp as the bare rcp.approx seed", ex[0]), ("sqrt without its final FMA", ex[1]), ("div without the remainder", div)):
+    for what, r in (("rcp as the bare rcp.approx seed", ex[0]), ("sqrt without its final FMA", ex[1]),
+                    ("sqrt without the scaling, subnormal x", ex[2]), ("div without the remainder", div)):
         rows.append(f"{what}: {r[2]} of {r[3]} not correctly rounded, worst {r[0]:.4g} ulp at 0x{r[1]:08x}")
     _show("planted mistakes", rows)
     assert sin[0] * U > COS_ABS_ERR and exp[0] > rl_ref.EXP_REL
-    assert ex[0][2] > 0 and ex[1][2] > 0 and div[2] > 0
+    assert ex[0][2] > 0 and ex[1][2] > 0 and ex[2][2] > 0 and div[2] > 0

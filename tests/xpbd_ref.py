@@ -378,14 +378,15 @@ def euler(j, parity):
     r10 = exact_scale(fsum([x * y, w * z]), 2)
     r20 = exact_scale(fsum([x * z, -(w * y)]), 2)
     psi, c0 = atan2(-r12, r22)
-    cth = sqrt(fsum([r00 * r00, r01 * r01]))
+    cth2 = fsum([r00 * r00, r01 * r01])
+    cth = sqrt(cth2)
     theta, c1 = atan2(r02, cth)
     phi, c2 = atan2(-r01, r00)
     zero = R(np.zeros_like(w.v))
     lon, _ = normalize((zero, r22, -r12))
     ax0 = (R(np.ones_like(w.v)), zero, zero)
     ax2 = (r02 * parity, r12 * parity, r22 * parity)
-    return dict(ang=(psi, theta, phi * parity), cut=(c0, c1, c2), ax=(ax0, lon, ax2), r10=r10, r20=r20)
+    return dict(ang=(psi, theta, phi * parity), cut=(c0, c1, c2), ax=(ax0, lon, ax2), r10=r10, r20=r20, cth2=cth2.v)
 
 
 def _slide_axis(k, parity, a_p, shape):
@@ -405,7 +406,7 @@ SITES = ("static friction", "sinking gate", "dist < 0", "dq.w >= 0", "atan2 cut 
 
 def positional_step(blob, states, actions, force=None, strict=True):
     """states [n, L, 13] fp32, actions [n, nu] fp32 -> dict(value [n, L, 13], radius [n, L, 13], undecided [n],
-    reasons {predicate: [n] mask}, sites {site: [n, L] mask})
+    reasons {predicate: [n] mask}, sites {site: [n, L] mask}, diag {name: [n, L] or [n, L, MAXCON] float64})
 
     A site is one predicate instance: (predicate, contact slot) for the three contact predicates, (predicate, dof) for the
     two atan2 cuts, (predicate,) for dq.w; its masks are per (sample, link).  `sites` holds the gated instances that made
@@ -426,6 +427,9 @@ def positional_step(blob, states, actions, force=None, strict=True):
     outcomes = {}
     infeasible = np.zeros(shape, dtype=bool)
     force = {} if force is None else force
+    # float64 values of the operands of the exact square roots and divisions (tests/tiny_families.py): the squared norms the
+    # step takes square roots of and the contact depth it divides
+    diag = {}
 
     def gate(name, mask, key=None):
         """marks the samples where a discontinuous predicate is within its radius and its outcomes jump"""
@@ -485,6 +489,7 @@ def positional_step(blob, states, actions, force=None, strict=True):
     a_p = qmul(qp, PQ)
     a_c = qmul(q, JQ)
     ea = euler(qmul(conj(a_p), a_c), parity)
+    diag["cth2 (acceleration)"] = ea["cth2"]
     jd = inv_rotate(vsub(w, wp), a_p)
     cad = m.lf(B.F_ANG_DAMP)
     rcw_s = rotate(RC, q)
@@ -545,6 +550,7 @@ def positional_step(blob, states, actions, force=None, strict=True):
         e = vwhere(is_slide, tuple(fsum([e[i], -(ak[i] * x)]) for i in range(3)), e)
     # P = n dl with n = e / |e|, dl = -|e| / (w_p + w_c + eps): P = -e / W, where W depends on the direction only through
     # |r x n|^2, so it stays inside [im_c + im_p + eps, that + |rc|^2 + ii_p |rp|^2] even where the direction is unknown
+    diag["anchor2"] = dot(e, e).v
     nrm, c = normalize(e)
     crc, crp = cross(rcw, nrm), cross(rpw, nrm)
     W = fsum([im_p, dot(crp, crp) * ii_p, im_c, dot(crc, crc), EPS])
@@ -557,6 +563,7 @@ def positional_step(blob, states, actions, force=None, strict=True):
     dq_p = tuple(exact_scale(x, -0.5) * ii_p for x in qmul(pure(cross(rpw, P)), qp))
     a_c = qmul(q, JQ)
     ea = euler(qmul(conj(a_p), a_c), parity)
+    diag["cth2 (joint solve)"] = ea["cth2"]
     err = []
     for k in range(B.MAXDOF):
         is_slide = ((smask >> k) & 1) == 1
@@ -597,6 +604,7 @@ def positional_step(blob, states, actions, force=None, strict=True):
         rad, mu = m.lf(base + 3), m.lf(base + 4)
         centre = vadd(p, rotate(S, q))
         dist = centre[2] - rad
+        diag.setdefault("dist", []).append(np.where(active, dist.v, np.nan))
         near = active & (np.abs(dist.v) <= dist.r)
         coll, coll_fm = forced(("dist < 0", ci), near, dist.v < 0)   # one outcome for the position and velocity stages
         cp = (centre[0], centre[1], centre[2] - fsum([rad, exact_scale(dist, 0.5)]))
@@ -606,6 +614,7 @@ def positional_step(blob, states, actions, force=None, strict=True):
         # static friction: cancel the tangential travel of the contact point since the start of the substep
         pbar = vadd(p_prev, rotate(inv_rotate(r, q), q_prev))
         dxy = (cp[0] - pbar[0], cp[1] - pbar[1], zero)
+        diag.setdefault("travel2", []).append(np.where(active & coll, dot(dxy, dxy).v, np.nan))
         # P_t = n_t dl_t with dl_t = -|dx| / (w_t + eps): P_t = -dx / W_t, W_t in [im + eps, im + eps + |r|^2]
         nt, ct = normalize(dxy)
         cr = cross(r, nt)
@@ -651,6 +660,7 @@ def positional_step(blob, states, actions, force=None, strict=True):
             rel = vadd(v0, cross(w0, r))
             vn = rel[2]
             tvec = (rel[0], rel[1], zero)
+            diag.setdefault("velocity2", []).append(np.where(active & coll, dot(tvec, tvec).v, np.nan))
             # P_d = -t min(fr, |v_t|) kd = -v_t s kd with s = min(fr / |v_t|, 1) in [0, 1]
             tdir, vtn = normalize(tvec)
             fr = rabs(dl) * mu * m.inv_dt
@@ -688,8 +698,9 @@ def positional_step(blob, states, actions, force=None, strict=True):
     undecided = np.zeros(n, dtype=bool)
     for m_ in reasons.values():
         undecided |= m_
+    diag = {k: np.stack(v, axis=-1) if isinstance(v, list) else v for k, v in diag.items()}
     return dict(value=value, radius=radius, undecided=undecided, reasons=reasons, sites=sites, outcomes=outcomes,
-                infeasible=infeasible)
+                infeasible=infeasible, diag=diag)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
